@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- GCUPS of the batched pairwise-alignment hot path on N B200s (BASELINE.json metric).
+"""bench.py -- GCUPS of the batched pairwise-alignment hot path on N H100s (BASELINE.json metric).
 
 A step = one pass of the hot path (K0 pack -> K1 fill -> K2 row-m/fix-ups/walk -> ops compaction, plus the one
 NCCL all-gather of result segments when N > 1) over one batch of synthetic pairs.
@@ -14,13 +14,13 @@ Headline workload at every N: BASELINE config 2 -- 1M pairs of 150x150 uniform r
              host memory (b2a_gathered_fetch) -- the gather and the reassembly are inside the timed region
   roofline : the K1 fill kernel against the int32-ALU roof (SURVEY 8d: 25 ops/cell local, 22 global/semiglobal/
              banded; peak = lane-ops/s measured in this run by b2a_util_int32_peak), with the HBM view beside it
-             (roofline.hbm: SURVEY 8d algorithmic bytes, and the DRAM traffic ncu measured)
+             (roofline.hbm: SURVEY 8d algorithmic bytes)
   configs  : the other BASELINE shapes on this GPU: C2 at 10k pairs (the north_star target), C3 (its 1/N share of
              100k pairs), C4 and C5 (the per-GPU share of the 8-GPU configuration), each with GCUPS, roofline
              fraction, fill shape and an oracle-checked sample
   verify   : (N > 1) the gathered segments decoded on rank 0 and compared with the oracle on a sample
-  cpu_baseline / --impl reference : the oracle (C++ restatement of rust-bio 4.0.1: rust-bio itself cannot be
-             built in this image) on the box's host cores, pinned threads, bounded sample
+  cpu_baseline / --impl reference : the oracle (C++ restatement of rust-bio 4.0.1: the build does not
+             compile rust-bio itself) on the host cores the process may use, pinned threads, bounded sample
 """
 from __future__ import annotations
 
@@ -55,6 +55,8 @@ def parse_args():
     ap.add_argument("--pairs", type=int, default=1_000_000, help="pairs per GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--configs", default="C2_10k,C3,C4,C5", help="extra configs to report ('' = none)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (N > 1: the gathered batch) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -64,11 +66,11 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region (read-only queries every 100 ms)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -157,7 +159,7 @@ def run_reference(args):
         "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": round(secs / args.steps * 1e3, 3), "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "int32", "data": "synthetic",
-        "config": {"workload": WORKLOAD, "note": "rust-bio cannot be built here (no rustc); this is the C++ "
+        "config": {"workload": WORKLOAD, "note": "the build does not compile rust-bio itself; this is the C++ "
                    "restatement of rust-bio 4.0.1 pinned to the reference's known-answer vectors"},
         "cpu_baseline": {"value": round(value, 4), "unit": "GCUPS", "cores": threads, "kind": "port",
                          "sample": f"{sample} pairs of {M}x{N_LEN} per step, {threads} pinned threads",
@@ -201,6 +203,28 @@ def check_sample(orc, mode_name, oscoring, batch, idx, res, threads):
             bad += 1
     return {"pairs_checked": int(len(idx)), "mismatches": bad, "ok": bad == 0,
             "what": "score, xstart, xend, ystart, yend and the operation vector vs the oracle"}
+
+
+def dump_outputs(out_dir, res):
+    """Write what a caller of the timed path receives (b2a_batch_fetch) as DIR/<name>.npy, at most ~45 MB: the
+    Alignment fields and op counts of every pair (a fixed, seeded sample of 2^20 pairs beyond that; `pairs` holds
+    their indices) and the operation vectors of a fixed sample of 16,384 of those (`ops_pairs`; `ops` concatenated,
+    `ops_off` the offsets, `clip_len` four per pair).  Values are integers below 2^24, exact in float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = res.n_pairs
+    rng = np.random.default_rng(20251015)
+    pairs = np.arange(n) if n <= 1 << 20 else np.sort(rng.choice(n, 1 << 20, replace=False))
+    lo, hi = res.ops_off[:n].astype(np.int64), res.ops_off[1:n + 1].astype(np.int64)
+    out = {f: getattr(res, f)[pairs].astype(np.float32) for f in ("score", "xstart", "xend", "ystart", "yend")}
+    out["n_ops"] = (hi - lo)[pairs].astype(np.float32)
+    out["pairs"] = pairs.astype(np.float64)
+    sample = pairs[np.sort(rng.choice(len(pairs), min(16384, len(pairs)), replace=False))]
+    out["ops_pairs"] = sample.astype(np.float64)
+    out["ops"] = np.concatenate([res.ops[lo[p]:hi[p]] for p in sample] + [np.zeros(0, np.uint8)]).astype(np.float32)
+    out["ops_off"] = np.concatenate([[0], np.cumsum(hi[sample] - lo[sample])]).astype(np.float64)
+    out["clip_len"] = res.clip_len[:4 * n].reshape(n, 4)[sample].astype(np.float32)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -320,7 +344,11 @@ def main():
         t[rank] = ms_total / steps
         dist.all_reduce(t)
         ms_ranks = [round(float(v), 4) for v in t.tolist()]
-    eng.fetch(None)
+    last = Results(P, ops_cap) if args.dump_outputs and world == 1 else None
+    eng.fetch(last)  # the results of the last timed step
+    if last is not None:
+        dump_outputs(args.dump_outputs, last)
+        del last
     st = eng.stats
     launches_step = int(st.kernel_launches) + (1 if world > 1 else 0)  # + the segment-header kernel
     # kernel-level numbers over instrumented passes (engine CUDA events on the same stream)
@@ -345,7 +373,10 @@ def main():
             orc.build()
             total_pairs = world * P
             allres, keep_all = pinned_results(torch, Results, total_pairs, 64 * total_pairs)
-            n_got, _ = eng.gathered_fetch(b["all"].data_ptr(), seg, world, allres)
+            n_got, _ = eng.gathered_fetch(b["all"].data_ptr(), seg, world, allres)  # the last timed step's gather
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, allres)
+
             rng = np.random.default_rng(7)
             bad, checked = 0, 0
             for r in range(world):
@@ -572,17 +603,9 @@ def main():
         # bytes out; the 4-bit traceback "fits on chip" in that accounting and is not counted
         algo_pair = (M + N_LEN) + 40 + (M + N_LEN + 4)
         algo_bytes = P * algo_pair
-        traffic = None
-        tsrc = None
-        tpath = os.path.join(ROOT, "profiles", "fill_traffic.json")
-        if os.path.exists(tpath):
-            with open(tpath) as f:
-                tj = json.load(f)
-            if tuple(tj.get("shape", (1, 16))) == (G, R):
-                traffic = int(tj["dram_bytes_per_pair"] * P)  # ncu dram read+write per pair x pairs of this launch
-                tsrc = tj.get("source", "profiles/fill_traffic.json (ncu --set full capture, scaled per pair)")
-        sm_max = (clocks or {}).get("sm_max_mhz") or 1965.0
-        nominal = 148 * 128 * sm_max * 1e6 / 1e12
+        n_sms = torch.cuda.get_device_properties(local).multi_processor_count
+        sm_max = (clocks or {}).get("sm_max_mhz") or 1980.0  # H100 SXM maximum SM clock
+        nominal = n_sms * 64 * sm_max * 1e6 / 1e12  # Hopper: 64 int32 lanes per SM
         k_all = float(np.mean(packs)) + fill_ms + float(np.mean(walks))
         roof = {"bound": "int32_alu", "kernel": f"fill_kernel<G={G},R={R},local> (K1: {100 * fill_ms / k_all:.0f}% of the step's kernel time)",
                 "achieved": round(fill_gcups * OPS_LOCAL / 1e3, 3), "peak": round(p_int, 3), "unit": "tera int32 lane-ops/s",
@@ -593,16 +616,13 @@ def main():
                                "SMs (tera lane-ops/s: add %.2f, minmax %.2f, mixed %.2f); the convention counts 25 plain ops per cell, the "
                                "kernel issues ~19 fused ones (DPX add-max, 3-way max)" % (fa.value, fb.value, fc.value),
                 "peak_nominal": round(nominal, 2), "frac_of_nominal": round(fill_gcups * OPS_LOCAL / 1e3 / nominal, 4),
-                "peak_nominal_source": "148 SMs x 128 int32 lanes x max SM clock",
-                "traffic": traffic, "traffic_source": tsrc,
+                "peak_nominal_source": f"{n_sms} SMs x 64 int32 lanes x max SM clock",
                 "hbm": {"bound": "hbm", "achieved": round(algo_bytes / (fill_ms * 1e-3) / 1e9, 2), "peak": hbm_peak, "unit": "GB/s",
                         "frac": round(algo_bytes / (fill_ms * 1e-3) / 1e9 / hbm_peak, 5), "peak_source": peak_src,
                         "algorithmic_bytes_per_launch": int(algo_bytes),
                         "algorithmic_bytes_per_pair": algo_pair,
-                        "traffic": traffic,
-                        "traffic_frac_of_peak": round(traffic / (fill_ms * 1e-3) / 1e9 / hbm_peak, 4) if traffic else None,
                         "note": "SURVEY 8d bytes: (m+n) in + 40 B record + (m+n+4) op bytes out, traceback on chip; the kernel "
-                                "itself streams its 4-bit traceback and strip-boundary rows through HBM (traffic)"}}
+                                "itself streams its 4-bit traceback and strip-boundary rows through HBM"}}
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
             from oracle import oracle as orc
@@ -620,7 +640,7 @@ def main():
             "vs_baseline": None, "dtype": "int32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "pairs_per_gpu": P, "m": M, "n": N_LEN,
                        "fill_shape": {"lanes_per_pair": G, "rows_per_lane": R},
-                       "l2": "inputs larger than L2: 320 MB staged sequences + ~12 GB traceback stream per step (126 MB L2)",
+                       "l2": "inputs larger than L2: 320 MB staged sequences + ~12 GB traceback stream per step (50 MB L2 on H100)",
                        "parallelism": (f"pair list sharded over {world} GPU(s); per step one NCCL all-gather of fixed-capacity result "
                                        f"segments ({gathered['bytes']} B received per rank) on a side stream, overlapping the next "
                                        f"step's kernels; no size agreement, no host sync in the timed region")

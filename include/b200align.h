@@ -1,6 +1,6 @@
 /*
  * b200align.h -- C ABI of libb200align.so: the drop-in boundary for the
- * `bio::alignment::pairwise` hot path of rust-bio 4.0.1, rebuilt B200-native.
+ * `bio::alignment::pairwise` hot path of rust-bio 4.0.1, rebuilt H100-native.
  *
  * The reference has no FFI for this path: its boundary is the Rust method
  * surface (reference src/alignment/pairwise/mod.rs):
@@ -302,7 +302,7 @@ int32_t b2a_gathered_fetch(b2a_engine* e, const void* dev_gathered, uint64_t seg
 int32_t b2a_compact_decode(const void* host_segment, uint64_t segment_bytes, uint64_t pair_base,
                            uint64_t ops_base, b2a_results* results, uint64_t* n_pairs, uint64_t* ops_bytes);
 
-/* ---- every visible GPU from ONE process (SURVEY 8b / 8e; what a Rust caller of the shim uses on an 8 x B200 box)
+/* ---- every visible GPU from ONE process (SURVEY 8b / 8e; what a Rust caller of the shim uses on an 8-GPU node)
  * b2a_multi_create: one engine + one stream per device (device_ids == NULL / n_devices <= 0: all visible devices)
  * and an NCCL communicator over them (ncclCommInitAll, libnccl.so.2 bound at run time).
  * b2a_multi_align_batch: Aligner::{custom,global,semiglobal,local} over a batch with HOST inputs and outputs -- the

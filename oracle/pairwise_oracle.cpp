@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE -- NOT PRODUCT CODE.
 //
 // CPU restatement ("oracle") of rust-bio 4.0.1 `bio::alignment::pairwise::Aligner`
-// (reference src/alignment/pairwise/mod.rs).  rust-bio cannot be compiled in this
-// image (no rustc/cargo), so this file restates the algorithm statement by
+// (reference src/alignment/pairwise/mod.rs).  The build does not compile rust-bio
+// (it needs no Rust toolchain), so this file restates the algorithm statement by
 // statement: same loop order (y outer, x inner), same strict comparisons, same
 // write order of every traceback store, same u16 row-major (m+1)x(n+1) traceback
 // matrix that is re-initialised on every call, same rolling two-column i32
@@ -446,7 +446,7 @@ double orc_align_batch(int mode, const orc_scoring* scoring, const uint8_t* blob
   if (threads < 1) threads = 1;
   auto t0 = std::chrono::steady_clock::now();
   // the CPUs this process may run on (cgroup / taskset aware); thread t is pinned to one of them so that the
-  // baseline does not depend on how the scheduler happens to migrate 128 threads (VERDICT r1: 1.2 vs 6.5 GCUPS
+  // baseline does not depend on how the scheduler happens to migrate 128 threads (1.2 vs 6.5 GCUPS
   // between two boxes with the same thread count)
   std::vector<int> cpus = orc_allowed_cpus();
   std::vector<std::thread> pool;

@@ -1,4 +1,4 @@
-"""rust_bio_b200: B200-native batched drop-in for rust-bio's `bio::alignment::pairwise` hot path.
+"""rust_bio_b200: H100-native batched drop-in for rust-bio's `bio::alignment::pairwise` hot path.
 
 Layout: csrc/ (CUDA kernels + C ABI, include/b200align.h), pairwise.py / alignment.py / scores.py
 (host-side mirror of the reference interface), engine.py (ctypes over the C ABI), synth.py

@@ -1,7 +1,7 @@
 """ctypes binding of rust_bio_b200/csrc/libb200align.so (C ABI: include/b200align.h).
 
 There is no Python or CPU implementation of the alignment behind this module: if the shared
-library is missing, or no sm_100 device is usable, the calls raise.
+library is missing, or no sm_90 (H100) device is usable, the calls raise.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Builds rust_bio_b200/csrc/libb200align.so in-tree with nvcc for sm_100a.
+"""Builds rust_bio_b200/csrc/libb200align.so in-tree with nvcc for sm_90a (H100).
 
 Usage: python -m rust_bio_b200.build [--force]
 The K1 fill kernel is instantiated once per (lanes-per-pair, rows-per-lane) shape in its own
@@ -21,11 +21,12 @@ SO = os.path.join(CSRC, "libb200align%s.so" % (("_" + VARIANT) if VARIANT else "
 SHAPES = [(1, 16), (1, 8), (1, 20), (2, 16), (2, 20), (4, 16), (8, 16), (8, 20), (32, 8), (32, 16)]
 # minimum resident CTAs per SM asked of ptxas per shape (__launch_bounds__): measured choice, see DESIGN.md
 MIN_BLOCKS = {(1, 16): int(os.environ.get("B2A_MINB_1_16", "3")), (8, 16): int(os.environ.get("B2A_MINB_8_16", "3")),
-              (8, 20): int(os.environ.get("B2A_MINB_8_20", "1"))}  # 8x20 at 3 CTAs/SM (168 registers) measured 10 % slower
+              (8, 20): int(os.environ.get("B2A_MINB_8_20", "1"))}  # 8x20 at 3 CTAs/SM (168 registers) was slower
 KS_DEFS = [f"-D{k}={os.environ[k]}" for k in ("B2A_KS_R", "B2A_KS_MINB") if os.environ.get(k)]  # strip-fill geometry knobs
 W_8_20 = os.environ.get("B2A_W_8_20")  # warps per CTA of the 8x20 fill (default in b2a_common.cuh)
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fwrapv", "--expt-relaxed-constexpr"] + ([f"-DB2A_W_8_20={W_8_20}"] if W_8_20 else []) + KS_DEFS
 HEADERS = ["b2a_common.cuh", "b2a_coop.cuh", "b2a_fill.cuh", "b2a_walk.cuh", "b2a_kernels.cuh", "b2a_plan.h", "b2a_banded.cuh", "b2a_banded_strip.cuh",
            "b2a_fill_launch.h", os.path.join("..", "..", "include", "b200align.h")]
@@ -47,6 +48,13 @@ def _run(cmd):
 
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OBJ, exist_ok=True)
+    stamp = os.path.join(OBJ, "flags.txt")  # objects built with other flags (another architecture) are rebuilt
+    want = " ".join([NVCC, *FLAGS]) + "\n"
+    if not os.path.exists(stamp):
+        force = True
+    else:
+        with open(stamp) as f:
+            force = force or f.read() != want
     hdrs = [os.path.join(CSRC, h) for h in HEADERS]
     jobs = []
     objs = []
@@ -77,7 +85,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 if verbose and log:
                     print(log, file=sys.stderr)
     if jobs or force or _stale(SO, objs):
-        _run([NVCC, "-shared", "-o", SO, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-ldl"])
+        _run([NVCC, "-shared", "-o", SO, *objs, *ARCH, "-ldl"])
+        with open(stamp, "w") as f:
+            f.write(want)
     return SO
 
 

@@ -1,4 +1,4 @@
-// Shared definitions of the B200 pairwise engine: device-side scoring, the
+// Shared definitions of the H100 pairwise engine: device-side scoring, the
 // per-block plan, scratch layouts and the closed-form DP boundaries.
 //
 // Reference being re-implemented: rust-bio 4.0.1 src/alignment/pairwise/mod.rs
@@ -174,7 +174,7 @@ B2A_HD int32_t xclip_score(const DevScoring& sc, int32_t j) {
 // Boundary-row index of (column j, pair pi) inside a block.  Fills with several pairs per warp (G < 32)
 // want [column][pair] (the warp's pairs touch one line per column); the warp-per-pair fill (G == 32)
 // reads/writes one pair's row column after column from a single lane, so [pair][column] keeps those
-// accesses inside cache lines (measured on C5: 408 -> 325 ms; the same layout for G = 8 cost C3 8 %).
+// accesses inside cache lines (faster on C5; the same layout for G = 8 was slower on C3).
 B2A_HD int64_t bnd_index(int32_t G, int32_t j, int32_t pi, int32_t maxn) {
   return G < 32 ? (int64_t)j * 32 + pi : (int64_t)pi * (maxn + 1) + j;
 }

@@ -1,6 +1,6 @@
 // libb200align.so: engine + C ABI (include/b200align.h).
 //
-// Host side of the B200 pairwise path: validates a batch the way the reference's
+// Host side of the H100 pairwise path: validates a batch the way the reference's
 // constructors do (mod.rs:517-518, 554-571), plans it (b2a_plan.h), moves it to
 // HBM and launches K0 (pack) -> K1 (fill) -> K2 (row m, fix-ups, walk) ->
 // ops compaction on one CUDA stream.  There is no CPU implementation of the
@@ -216,13 +216,13 @@ void choose_shape(const b2a_engine* e, uint32_t maxm, uint32_t maxn, uint64_t n_
     return;
   }
   const uint64_t stage1 = (uint64_t)((maxm + 15) / 16 * 16 + 64 + (maxn + 15) / 16 * 16 + 64) * 32 * fill_warps_of(1, 16);
-  if (n_pairs >= 49152 && stage1 <= kMaxStageSmem && maxm <= 2048) {  // measured: 8x20 wins below ~50k reads of 150
+  if (n_pairs >= 49152 && stage1 <= kMaxStageSmem && maxm <= 2048) {  // 8x20 is the faster shape below ~50k reads of 150
     *G = 1;
     *R = 16;
   } else if ((n_pairs >= 4096 && maxm <= 4096) || maxm <= 161) {
     // four pairs to a warp: enough warps to fill the GPU (or a single strip anyway).  128-row or 160-row
-    // strips, whichever pads the rows less: 10k reads of 150 run as one strip of 8x20 (7 % padding) at
-    // 0.34 ms against 0.46 (2x16), 0.52 (8x16: two strips) and 0.68 (32x8) -- profiles/r02_small_batch_shapes.txt
+    // strips, whichever pads the rows less: 10k reads of 150 run as one strip of 8x20 (7 % padding), faster
+    // than 2x16, 8x16 (two strips) or 32x8
     const uint64_t rows = maxm > 1 ? maxm - 1 : 1;
     const uint64_t pad16 = (rows + 127) / 128 * 128, pad20 = (rows + 159) / 160 * 160;
     *G = 8;
@@ -255,7 +255,7 @@ int validate_scoring(b2a_engine* e, const b2a_scoring* s) {
 
 extern "C" {
 
-const char* b2a_version(void) { return "b200align 0.1 (sm_100a)"; }
+const char* b2a_version(void) { return "b200align 0.1 (sm_90a)"; }
 
 const char* b2a_last_error(const b2a_engine* e) { return e ? e->err.c_str() : "null engine"; }
 
@@ -268,12 +268,11 @@ int32_t b2a_engine_create(b2a_engine** out, int32_t device_id) {
   if (cudaSetDevice(device_id) != cudaSuccess) return B2A_E_NO_DEVICE;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device_id) != cudaSuccess) return B2A_E_NO_DEVICE;
-  if (prop.major < 10) return B2A_E_NO_DEVICE;  // kernels are built for sm_100a only
+  if (prop.major != 9 || prop.minor != 0) return B2A_E_NO_DEVICE;  // kernels are built for sm_90a (H100) only
   b2a_engine* e = new b2a_engine();
   e->device = device_id;
   e->num_sms = prop.multiProcessorCount;
-  // (measured on 10k reads: K1 at 67 % issue and K2 at 36 % are both instruction-bound, and K2's CTAs displace K1's
-  //  register-heavy ones: 0.571 ms overlapped against 0.558 ms back to back -- off unless asked for)
+  // (K2's CTAs displace K1's register-heavy ones: off unless asked for)
   e->overlap_small = false;
   if (const char* env = getenv("B2A_BANDED_LITERAL")) e->banded_fast = atoi(env) == 0;
   if (const char* env = getenv("B2A_BANDED_STRIP")) e->banded_strip = atoi(env) != 0;
@@ -787,16 +786,15 @@ int32_t b2a_batch_run(b2a_engine* e) {
     wp.clip_len = e->d_clip.as<uint32_t>();
     wp.status = e->d_status.as<uint32_t>();
     wp.err_flag = ctl + 1;
-    // (running K2 inside K1's warps was measured: 28.4 ms vs 22.4 + 3.2 ms separately -- the latency-bound
-    //  walk holds one of only 12 resident warps per SM; K2 stays its own launch)
+    // (K2 inside K1's warps was slower: K2 stays its own launch)
     const bool fuse = false;
     fp.task_limit = (pl.G == 32) ? 0u : e->fill_task_limit;  // strip-pipelined tasks need the persistent grid
     const uint64_t wave_pairs = (uint64_t)nb * 32;
     const bool warp_walk = e->walk_mode == 2 || (e->walk_mode == 0 && wave_pairs <= kWarpWalkMaxPairs);
     uint32_t per_warp_smem = 0;
     // warps (pairs of one 32-pair block) per CTA of the warp-per-pair K2: the block's scratch is laid out
-    // [index][pair], so the pairs of a CTA share the sectors they read through L1
-    // (10k reads: 8 warps 0.134 ms, 4 warps 0.159, 16 warps 0.142, 32 warps 0.155 -- profiles/r02_10k_target.txt)
+    // [index][pair], so the pairs of a CTA share the sectors they read through L1 (8 warps measured best on 10k
+    // reads against 4, 16 and 32)
     uint32_t wcta_warps = e->walk_cta_warps;
     if (warp_walk) {
       // the pair's x and y are copied into shared memory when the CTA's pairs' worth fits its budget
@@ -818,8 +816,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     const bool overlap = overlap_big || (e->overlap_small && pl.waves.size() == 1 && warp_walk && pl.G != 32 && nb >= 64 &&
                                          !use_tail && e->walk_mode != 1);
     // Tail-aware split (small batches of equal tasks): the persistent fill runs whole rounds of one task per
-    // resident warp; what is left over is a thin last round (10k reads on 8x20: 2,500 tasks on 1,184 warps = two
-    // rounds + 132 tasks that take 0.07 ms with the SMs 7/8 idle).  The pairs of the whole rounds (A) and the
+    // resident warp; what is left over is a thin last round that runs with most SMs idle.  The pairs of the whole rounds (A) and the
     // remainder (B) are filled back to back, and K2 of A runs beside the fill of B: B's few CTAs go out on the
     // high-priority stream first, A's walk takes the rest of the GPU.
     uint32_t split_b = 0;  // blocks of part A (0: no split)
@@ -831,7 +828,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
       if (slots > 0 && tasks > slots) {
         const uint32_t rounds = tasks / slots, rem = tasks % slots;
         const uint32_t a_blocks = (uint32_t)((uint64_t)rounds * slots / (uint32_t)pl.G);
-        // (measured: 10k reads, a remainder of 0.11 rounds: 0.506 -> 0.464 ms; 7k reads, 0.48 rounds: 0.391 -> 0.411)
+        // (a remainder of a tenth of a round gained; half a round lost: at most a quarter)
         if (rem > 0 && rounds <= 6 && rem * 4 <= slots && a_blocks > 0 && a_blocks < nb) split_b = a_blocks;
       }
     }
@@ -865,9 +862,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[1], st));
       CK(cudaEventRecord(e->sub_ev[0], st));  // fill A done
       // fill B + walk B on the high-priority stream, walk A on the auxiliary one
-      // (measured, profiles/r02_10k_target.txt: beside walk A the fill of B takes 144 us instead of 86 -- walk A's 64
-      //  resident warps per SM crowd it -- so B's chain, +186 us, ends the step; walk A at a quarter of its occupancy
-      //  frees B (+100 us) but then takes +246 us itself; swapping the stream priorities changes nothing)
+      // (walk A's resident warps slow the fill of B, so B's chain ends the step)
       cudaStream_t sB = e->tail_stream, sA = e->aux_stream;
       CK(cudaStreamWaitEvent(sB, e->sub_ev[0], 0));
       CK(cudaStreamWaitEvent(sA, e->sub_ev[0], 0));
@@ -1112,15 +1107,14 @@ static int32_t align_batch_pipelined(b2a_engine* e, int32_t mode, const b2a_scor
   // while the first chunk is staged and the host idles while the last one drains)
   uint64_t K = (uint64_t)e->pipe_chunks;
   // A small first chunk (its H2D is exposed), then growing ones (each chunk costs a fill tail of about half
-  // a warp-task), and a smaller last one (its walk and D2H are exposed).  Measured on 1M x 150x150:
-  // 1,3,6,6,3 -> 28.4-29.5 ms against 31.7 ms for 1,2,2,2,1 (profiles/r01_e2e_chunk_schedules.txt).
+  // a warp-task), and a smaller last one (its walk and D2H are exposed): on 1M x 150x150, 1,3,6,6,3 measured
+  // faster than 1,2,2,2,1.
   std::vector<double> wts(K, 6.0);
   wts[0] = 1.0;
   if (K >= 3) wts[1] = 3.0;
   wts[K - 1] = K >= 4 ? 3.0 : 2.0;
-  // three slots (round 2): the last chunk's walk and copies hide under nothing, but its fill no longer waits for
-  // a slot, so equal late chunks measure best: 1,3,5,5,5 -> 26.9 ms per 1M-pair call against 27.3 for 1,3,6,6,3
-  // (profiles/r02_e2e_chunk_schedules.txt)
+  // three slots: the last chunk's walk and copies hide under nothing, but its fill no longer waits for a slot,
+  // so equal late chunks measure best (1,3,5,5,5 against 1,3,6,6,3)
   if (K == 5) wts = {1.0, 3.0, 5.0, 5.0, 5.0};
   if (const char* env = getenv("B2A_PIPE_WEIGHTS")) {  // development knob: comma-separated chunk weights
     std::vector<double> w2;

@@ -192,8 +192,10 @@ constexpr int32_t KEY_NONE = (int32_t)0x80000000;
 //    smaller S/D of column j-1; column 0 is non-increasing in i), and they sit at higher row indices, so they can
 //    never win the column tracker's first-maximum: no per-row mask is needed there;
 //  * the writer needs (S, I) of row m-1 = the partial lane's row rv-1.  CAPQ >= 0: uniform block, that row is
-//    known to lie in row-quad CAPQ (compile time), so only four rows carry the capture compare; CAPQ == R/4: no
-//    lane of the strip is partial; CAPQ == -1: ragged block, every row compares.
+//    known to lie in row-quad CAPQ (compile time), so only four rows carry the capture test; CAPQ == R/4: no
+//    lane of the strip is partial; CAPQ == -1: ragged block, every row tests.  The test reads one bit of a one-hot
+//    mask built once per column step: written as r == rv - 1 in each unrolled row, optimised sm_90a code of the
+//    non-last-column instantiation captured the lane's bottom row instead (bit-exact only at ptxas -O0).
 template <int G, int R, int FLAGS, bool MASKED, bool LAST, int CAPQ>
 B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tstep, const int32_t q, const int32_t rowbase,
                         const int32_t rv, int32_t (&Sp)[R], int32_t (&Dp)[R], int32_t (&SnR)[R],
@@ -222,6 +224,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
   const int32_t cj = 4095 - (PR ? (tstep & KREL_MASK) : j);
   const int32_t one = c.one, k2 = one + one, k16 = k2 * 8, k1024 = k16 * 64;
   const int32_t q4 = q * 4;
+  const uint32_t capbit = (MASKED && rv >= 1) ? 1u << (rv - 1) : 0u;  // one-hot: the lane's row m-1
   int32_t Tl = KEY_NONE;        // packed column tracker of this lane's rows (local row index)
   int32_t key_even = KEY_NONE;
   int32_t sdo = fmad(sdiag, one, go4d);  // diagonal S, open-biased
@@ -287,7 +290,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
       c.rows[ROWS_NL * c.rows_pad * 32 + slot] = nib;
     }
     if (MASKED && (CAPQ < 0 || (r >> 2) == CAPQ)) {
-      if (r == rv - 1) {
+      if ((capbit >> r) & 1u) {
         cap_s = s4;
         cap_i = i4;
       }

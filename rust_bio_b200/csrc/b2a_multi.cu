@@ -1,4 +1,4 @@
-// Multi-GPU form of the path behind the C ABI (SURVEY 8b / 8e): ONE process drives every visible B200.
+// Multi-GPU form of the path behind the C ABI (SURVEY 8b / 8e): ONE process drives every visible GPU.
 //
 // The reference has no distributed layer; pairs are independent, so the batch is split contiguously over the
 // devices (equal counts), every device runs K0..K2 on its share from its own stream, and ONE ncclAllGather of

@@ -1,4 +1,4 @@
-// Measured int32 ALU peak (SURVEY 8d: "P_int32 measured on the box ... a committed microbenchmark of
+// Measured int32 ALU peak (SURVEY 8d: "P_int32 measured on the GPU ... a committed microbenchmark of
 // independent IADD3 / VIMNMX chains over all SMs").  Measurement infrastructure for bench.py's
 // int32 roofline; not on the alignment path.
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Mirror of `bio::alignment::pairwise` (reference src/alignment/pairwise/mod.rs) on the B200 engine.
+"""Mirror of `bio::alignment::pairwise` (reference src/alignment/pairwise/mod.rs) on the H100 engine.
 
 Same names, argument meaning and error behaviour as the reference:
   MIN_SCORE (mod.rs:174), MatchParams (186-217), Scoring (238-429), Aligner (472-1015).

@@ -2,7 +2,7 @@
 //! this crate's `*_batch` methods (libb200align.so), with the same splitmix64 generator as
 //! `rust_bio_b200/synth.py` (SURVEY 8d) so both sides and the Python/C++ harness see identical sequences.
 //!
-//! NOT COMPILED IN THIS REPOSITORY'S BUILD IMAGE (no Rust toolchain there): it ships so that the real crate can be
+//! NOT COMPILED BY THIS REPOSITORY'S BUILD (it needs no Rust toolchain): it ships so that the real crate can be
 //! timed wherever one exists.  Workload shape follows rust-bio's own benches/pairwise.rs:140-159
 //! (`Aligner::with_capacity(..).local/global/semiglobal`, score 1/-1, gap_open -5, gap_extend -1).
 //!

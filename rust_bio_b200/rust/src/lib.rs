@@ -1,6 +1,6 @@
-//! `bio_b200::alignment::pairwise` -- the rust-bio 4.0.1 pairwise API on a B200.
+//! `bio_b200::alignment::pairwise` -- the rust-bio 4.0.1 pairwise API on an H100.
 //!
-//! NOT COMPILED IN THIS REPOSITORY'S BUILD IMAGE (no Rust toolchain there).  It is the binding a
+//! NOT COMPILED BY THIS REPOSITORY'S BUILD (it needs no Rust toolchain).  It is the binding a
 //! maintainer adds next to `bio`: same type and method names as
 //! `bio::alignment::pairwise::{MIN_SCORE, MatchFunc, MatchParams, Scoring, Aligner}`
 //! (rust-bio src/alignment/pairwise/mod.rs:174-1015) plus `*_batch` methods; every method goes
@@ -290,11 +290,11 @@ pub mod alignment {
                 let mut engine: *mut c_void = std::ptr::null_mut();
                 let device = std::env::var("B2A_DEVICE").ok().and_then(|v| v.parse().ok()).unwrap_or(0);
                 let rc = unsafe { b2a_engine_create(&mut engine, device) };
-                assert!(rc == 0, "b200align: no usable sm_100 device (rc = {}); there is no CPU fallback", rc);
+                assert!(rc == 0, "b200align: no usable sm_90 (H100) device (rc = {}); there is no CPU fallback", rc);
                 Aligner { scoring, engine, multi: std::ptr::null_mut() }
             }
 
-            /// Use every visible B200 for the `*_batch` methods (not part of rust-bio's API: its Aligner is a
+            /// Use every visible GPU for the `*_batch` methods (not part of rust-bio's API: its Aligner is a
             /// single-threaded CPU object).  Panics if the devices cannot be opened.
             pub fn on_all_gpus(mut self) -> Self {
                 let mut m: *mut c_void = std::ptr::null_mut();

@@ -29,7 +29,7 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_no_cpu_fallback_without_device():
-    """On a box without a usable sm_100 device the engine refuses to exist (no CPU path)."""
+    """On a machine without a usable sm_90 (H100) device the engine refuses to exist (no CPU path)."""
     import torch
     from rust_bio_b200 import _lib
     if torch.cuda.is_available():

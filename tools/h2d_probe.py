@@ -1,4 +1,4 @@
-"""Pinned host<->device copy bandwidth of the box (what bounds the e2e arm), and the CPU quota the container sees."""
+"""Pinned host<->device copy bandwidth of the machine (what bounds the e2e arm), and the CPU quota the process sees."""
 import torch, time
 for mb in (64, 359):
     h = torch.empty(mb << 20, dtype=torch.uint8).pin_memory()

@@ -1,5 +1,5 @@
-"""Dev tool: condense an .ncu-rep (ncu --set full) into the per-kernel metrics quoted in DESIGN.md / profiles/.
-usage: python tools/ncu_summary.py report.ncu-rep > profiles/<name>.txt"""
+"""Dev tool: condense an .ncu-rep (ncu --set full) into per-kernel metrics.
+usage: python tools/ncu_summary.py report.ncu-rep > <name>.txt"""
 import csv, subprocess, sys
 KEEP = [
     "gpu__time_duration.sum", "launch__grid_size", "launch__block_size", "launch__registers_per_thread",
