@@ -18,6 +18,7 @@ struct int4 { int x, y, z, w; };
 struct int2 { int x, y; };
 struct uint4 { unsigned x, y, z, w; };
 inline int4 make_int4(int x, int y, int z, int w) { return int4{x, y, z, w}; }
+inline int2 make_int2(int x, int y) { return int2{x, y}; }
 #endif
 
 namespace b2a {
@@ -80,6 +81,9 @@ enum : int {
   F_PACKREL = 128,   // long sequences (m or n > 4095, |S| < 2^18): the same packed keys with RELATIVE indices -- the row
                      // tracker's column inside a chunk of 2^KREL_BITS columns (flushed to the rows arena at each chunk
                      // end), the column tracker's row inside the strip (made absolute where the strip hands it on)
+  F_BND8 = 256,      // with F_PACKTRK: the strip boundary record is 8 bytes, int2 {(I4 << 16) | (S4 & 0xffff), packed
+                     // column-tracker key}, instead of int4 {S4, I4, key, row}.  Needs every S4 = 4*S and I4 = 4*I + 2
+                     // to fit a signed 16-bit half: 4*score_bound + 3 < 2^15 (boundary8_ok in b2a_plan.h)
 };
 #ifndef B2A_KREL_BITS
 #define B2A_KREL_BITS 12  // (a test build shortens the chunks to exercise the flushes on small inputs)
@@ -109,7 +113,7 @@ struct Block {
   uint32_t K;        // 8-column traceback groups per strip: ceil((maxn + G - 1) / 8)
   uint32_t rows_pad; // row slots in the rows arena: nstrips*G*R + 2
   uint64_t seq_off;  // bytes into the staged-sequence arena (x tasks, then y tasks)
-  uint64_t bnd_off;  // bytes into the boundary arena: (maxn+1) * 32 * 16
+  uint64_t bnd_off;  // bytes into the boundary arena: (maxn+1) * 32 * 16, or (maxn+1) * 32 * 8 under F_BND8
   uint64_t rows_off; // bytes into the rows arena: 5 arrays of rows_pad*32 int32
   uint64_t rowm_off; // bytes into the row-m arena: (maxn+1)*32 bytes
   uint64_t tb_off;   // bytes into the traceback arena: G * nstrips * K * TBW * 512
@@ -178,6 +182,17 @@ B2A_HD int32_t xclip_score(const DevScoring& sc, int32_t j) {
 B2A_HD int64_t bnd_index(int32_t G, int32_t j, int32_t pi, int32_t maxn) {
   return G < 32 ? (int64_t)j * 32 + pi : (int64_t)pi * (maxn + 1) + j;
 }
+
+// F_BND8 record word: lo and hi as two signed 16-bit halves (both must fit, see F_BND8)
+B2A_HD int32_t pack_s16x2(int32_t lo, int32_t hi) {
+#if defined(__CUDA_ARCH__)
+  return (int32_t)__byte_perm((uint32_t)lo, (uint32_t)hi, 0x5410);  // one PRMT
+#else
+  return (int32_t)(((uint32_t)hi << 16) | ((uint32_t)lo & 0xffffu));
+#endif
+}
+B2A_HD int32_t lo_s16(int32_t w) { return (int32_t)(int16_t)(uint16_t)((uint32_t)w & 0xffffu); }
+B2A_HD int32_t hi_s16(int32_t w) { return w >> 16; }
 
 // K1's scaled LUT: alpha real rows of alpha entries, then one poison row (the substitution "score" gap_open for
 // every y symbol, i.e. the entry 4*go + 3 - (4*go + 1) = 2) that the padded rows of a masked strip read

@@ -547,6 +547,7 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
   e->sc = sc;
   e->flags = scoring_flags(sc, score_bound, maxm, maxn);
   if (e->no_packrel) e->flags &= ~F_PACKREL;  // (test knob: the explicit (value, index) trackers for long sequences)
+  if (boundary8_ok(e->flags, score_bound)) e->flags |= F_BND8;  // half the strip-boundary bytes of K1 and K2
 
   return B2A_OK;
 }
@@ -608,7 +609,7 @@ int32_t b2a_batch_stage(b2a_engine* e, int32_t mode, const b2a_scoring* s, const
   for (int attempt = 0;; ++attempt) {
     e->shape = find_shape(G, R);
     if (!e->shape) return e->fail(B2A_E_INVALID, "no fill kernel for the requested shape");
-    build_plan(e->plan, pairs->x_len, pairs->y_len, n, G, R, budget);
+    build_plan(e->plan, pairs->x_len, pairs->y_len, n, G, R, budget, e->flags);
     if (64 + lut_bytes + (uint64_t)fill_warps_of(G, R) * e->plan.smem_seq_bytes <= kMaxStageSmem) break;
     // Shapes with several pairs per warp stage 32/G whole (x, y) per warp; long sequences (a read against a
     // 15 kb reference ...) only fit the warp-per-pair shape, which stages one strip of x and one y per warp
@@ -775,6 +776,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     wp.G = pl.G;
     wp.R = pl.R;
     wp.packtrk = (e->flags & F_PACKTRK) ? 1 : 0;
+    wp.bnd8 = (e->flags & F_BND8) ? 1 : 0;
     wp.filter_clips = (e->mode == B2A_MODE_SEMIGLOBAL || e->mode == B2A_MODE_LOCAL) ? 1 : 0;
     wp.score = e->d_score.as<int32_t>();
     wp.xstart = e->d_xs.as<uint32_t>();

@@ -64,7 +64,7 @@ struct LaneCtx {
   int32_t K;
   int32_t rows_pad;
   bool uniform;
-  int4* bnd;             // block base, [column][32]
+  int4* bnd;             // block base, [column][32] (bnd_index); F_BND8: the same bytes as int2 records
   int32_t* rows;         // block base, ROWS_ARRAYS arrays of [rows_pad][32]
   uint4* tb;             // task base: [strip][k][q][32]
   uint32_t lut_base;     // device: shared-space byte address of the LUT; host sim: 0
@@ -168,7 +168,8 @@ B2A_HD uint32_t ld_progress(const uint32_t* p) {
   return *p;
 #endif
 }
-B2A_HD int4 ld_boundary(const int4* p, bool bypass_l1) {
+template <class T>  // int4 or int2 (F_BND8) records
+B2A_HD T ld_boundary(const T* p, bool bypass_l1) {
 #if defined(__CUDA_ARCH__)
   return bypass_l1 ? __ldcg(p) : *p;
 #else
@@ -316,8 +317,11 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
   constexpr bool LUT = (FLAGS & F_LUT) != 0;
   constexpr bool PR = (FLAGS & F_PACKREL) != 0;
   constexpr bool PK = (FLAGS & F_PACKTRK) != 0 || PR;  // packed keys in the lanes (PR: relative indices)
+  constexpr bool B8 = (FLAGS & F_BND8) != 0;           // 8-byte boundary record (with F_PACKTRK only)
+  static_assert(!B8 || ((FLAGS & F_PACKTRK) != 0 && !PR), "F_BND8 needs the packed column tracker with absolute rows");
   constexpr int P = 32 / G;
   constexpr int TBW = tbw_of(R);
+  int2* const bnd8 = reinterpret_cast<int2*>(c.bnd);
   const int32_t m = c.m, n = c.n;
   const int32_t rowbase = s * (G * R) + c.l * R;  // row above this lane's first row
   // valid rows of this lane: rows <= m-1
@@ -387,6 +391,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
     }
   };
   int4 pre = make_int4(0, 0, 0, 0);
+  int2 pre8 = make_int2(0, 0);  // B8: the record as loaded, unpacked where it is used (the load stays a prefetch)
   const bool top_from_mem = (c.l == 0) && (s > 0);
   const bool top_from_row0 = (c.l == 0) && (s == 0);
   // strip-pipelined: number of columns the strip above has published so far
@@ -404,7 +409,8 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
   const bool top_valid = top_from_mem && rv >= 1;  // a strip without valid rows needs no boundary (ragged blocks)
   if (top_valid && n >= 1) {
     wait_col(1);
-    pre = ld_boundary(&c.bnd[bnd_index(G, 1, c.pi, c.maxn)], piped);
+    if (B8) pre8 = ld_boundary(&bnd8[bnd_index(G, 1, c.pi, c.maxn)], piped);
+    else pre = ld_boundary(&c.bnd[bnd_index(G, 1, c.pi, c.maxn)], piped);
   }
   const bool writer =
       MASKED ? (rv >= 1 && (c.l == G - 1 || rowbase + R >= m - 1)) : (c.l == G - 1);
@@ -448,9 +454,19 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
           up_ti = m;
         }
       } else if (top_from_mem) {  // the boundary row is kept in the fill's own scaled domain
-        in_s = pre.x;
-        in_i = pre.y;
-        if (TC) {
+        if (B8) {  // {S4 | I4 << 16, key}: the row index of a packed key is inside the key
+          in_s = lo_s16(pre8.x);
+          in_i = hi_s16(pre8.x);
+          // the key is copied out (an IMAD ptxas cannot fold) so that both halves of pre8 are dead before the
+          // prefetch below: the load then writes pre8's registers directly.  Left as a plain use, the key stays
+          // live to the column's end and ptxas loads into a second pair and moves the new value over at once,
+          // waiting out the load's latency in every column.
+          if (TC) in_tv = fmad(pre8.y, c.one, 0);
+        } else {
+          in_s = pre.x;
+          in_i = pre.y;
+        }
+        if (TC && !B8) {
           if (PR) {  // unpacked (value, row) of the strips above; this strip's own key starts empty
             up_tv = pre.z;
             up_ti = pre.w;
@@ -462,7 +478,8 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
         }
         if (j < n && top_valid) {  // prefetch next column's boundary
           wait_col(j + 1);
-          pre = ld_boundary(&c.bnd[bnd_index(G, j + 1, c.pi, c.maxn)], piped);
+          if (B8) pre8 = ld_boundary(&bnd8[bnd_index(G, j + 1, c.pi, c.maxn)], piped);
+          else pre = ld_boundary(&c.bnd[bnd_index(G, j + 1, c.pi, c.maxn)], piped);
         }
       }
       int32_t sup = in_s, iup = in_i, Tv = in_tv, Ti = in_ti;
@@ -475,27 +492,32 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       }
       sup_prev = in_s;
       if (writer) {
-        int4 o;  // decoded by decode_boundary() in b2a_walk.cuh
-        o.x = (MASKED && rv < R) ? cap_s : sup;  // a full lane's row m-1 is its bottom row
-        o.y = (MASKED && rv < R) ? cap_i : iup;
-        o.z = TC ? Tv : t_none;
-        o.w = TC ? Ti : m;
-        if (PR) {  // the boundary row leaves the strip unpacked, as K2 and the strip below read it
-          o.z = NEG4;
-          o.w = m;
-          if (TC) {
-            o.z = up_tv;
-            o.w = up_ti;
-            if (Tv != KEY_NONE) {
-              const int32_t loc_v = ((Tv >> 12) << 2) + xs4_pr;  // 4 * (S + xs)
-              if (loc_v > up_tv) {
-                o.z = loc_v;
-                o.w = s * (G * R) + (4095 - (Tv & 4095));
+        if (B8) {  // one PRMT and one 64-bit store
+          const int32_t s4 = (MASKED && rv < R) ? cap_s : sup, i4 = (MASKED && rv < R) ? cap_i : iup;
+          bnd8[bnd_index(G, j, c.pi, c.maxn)] = make_int2(pack_s16x2(s4, i4), TC ? Tv : t_none);
+        } else {
+          int4 o;  // decoded by decode_boundary() in b2a_walk.cuh
+          o.x = (MASKED && rv < R) ? cap_s : sup;  // a full lane's row m-1 is its bottom row
+          o.y = (MASKED && rv < R) ? cap_i : iup;
+          o.z = TC ? Tv : t_none;
+          o.w = TC ? Ti : m;
+          if (PR) {  // the boundary row leaves the strip unpacked, as K2 and the strip below read it
+            o.z = NEG4;
+            o.w = m;
+            if (TC) {
+              o.z = up_tv;
+              o.w = up_ti;
+              if (Tv != KEY_NONE) {
+                const int32_t loc_v = ((Tv >> 12) << 2) + xs4_pr;  // 4 * (S + xs)
+                if (loc_v > up_tv) {
+                  o.z = loc_v;
+                  o.w = s * (G * R) + (4095 - (Tv & 4095));
+                }
               }
             }
           }
+          c.bnd[bnd_index(G, j, c.pi, c.maxn)] = o;
         }
-        c.bnd[bnd_index(G, j, c.pi, c.maxn)] = o;
         if (piped && ((j & 15) == 0 || j == n)) {  // publish (release) every 16 columns and at the end
           fence_device();
           *reinterpret_cast<volatile uint32_t*>(c.prog_mine) = (uint32_t)j;

@@ -62,6 +62,12 @@ cudaError_t B2A_CAT(launch_fill_, B2A_G, B2A_R)(int flags, const FillParams& prm
     B2A_CASE(F_LUT | ALL | F_PACKTRK)
     B2A_CASE(F_LUT | ALL | F_RELU)
     B2A_CASE(F_LUT | ALL | F_PACKTRK | F_RELU)
+    B2A_CASE(F_TRACK_ROWS | F_PACKTRK | F_BND8)
+    B2A_CASE(ALL | F_PACKTRK | F_BND8)
+    B2A_CASE(ALL | F_PACKTRK | F_RELU | F_BND8)
+    B2A_CASE(F_LUT | F_TRACK_ROWS | F_PACKTRK | F_BND8)
+    B2A_CASE(F_LUT | ALL | F_PACKTRK | F_BND8)
+    B2A_CASE(F_LUT | ALL | F_PACKTRK | F_RELU | F_BND8)
     B2A_CASE(F_TRACK_ROWS | F_PACKREL)
     B2A_CASE(ALL | F_PACKREL)
     B2A_CASE(ALL | F_PACKREL | F_RELU)

@@ -35,8 +35,10 @@ struct Plan {
 
 inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 
+// `flags`: the fill's kernel flags (F_BND8 halves the boundary record)
 inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, uint64_t n_pairs, int G,
-                       int R, uint64_t tb_budget) {
+                       int R, uint64_t tb_budget, int flags = 0) {
+  const uint64_t bnd_rec = (flags & F_BND8) ? 8 : 16;
   p.G = G;
   p.R = R;
   p.n_pairs = n_pairs;
@@ -93,7 +95,7 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     // the warp-per-pair shape runs (pair, strip) tasks that stage one strip of x (b2a_fill.cuh)
     const uint32_t stage_x = G == 32 ? (uint32_t)(G * R) : k.xwords * P * 4;
     p.smem_seq_bytes = std::max<uint32_t>(p.smem_seq_bytes, stage_x + k.ywords * P * 4);
-    const uint64_t bnd = align_up((uint64_t)(k.maxn + 1) * 32 * 16, 256);
+    const uint64_t bnd = align_up((uint64_t)(k.maxn + 1) * 32 * bnd_rec, 256);
     const uint64_t rows = align_up((uint64_t)ROWS_ARRAYS * k.rows_pad * 32 * 4, 256);
     const uint64_t rowm = align_up((uint64_t)(k.maxn + 1) * 32 * 2, 256);
     const uint64_t tb = align_up((uint64_t)G * k.nstrips * k.K * TBW * 512, 256);
@@ -151,6 +153,14 @@ inline int scoring_flags(const DevScoring& sc, int64_t score_bound = (1ll << 40)
   else if ((f & (F_TRACK_ROWS | F_TRACK_COLS)) && score_bound < (1ll << 18))
     f |= F_PACKREL;  // longer sequences: the packed keys with chunk- / strip-relative indices
   return f;
+}
+
+// Whether the fill may use the 8-byte strip boundary record (F_BND8) on top of `flags` = scoring_flags(...):
+// the packed-tracker form only (its record carries no row index), and every S4 / I4 of the record within a signed
+// 16-bit half.  Fills without trackers (global), the long-sequence form (F_PACKREL) and the explicit (value, row)
+// trackers keep the 16-byte record.
+inline bool boundary8_ok(int flags, int64_t score_bound) {
+  return (flags & F_PACKTRK) != 0 && 4 * score_bound + 3 < (1ll << 15);
 }
 
 }  // namespace b2a

@@ -33,6 +33,7 @@ struct WalkParams {
   int32_t G, R;
   int32_t filter_clips;  // semiglobal / local: Alignment::filter_clip_operations
   int32_t packtrk;       // K1 ran with F_PACKTRK (how the column tracker in the boundary row is encoded)
+  int32_t bnd8;          // K1 ran with F_BND8 (8-byte boundary records)
   uint32_t seq_smem_per_warp;  // warp-per-pair K2: bytes of shared memory per warp for the pair's x and y (0: none)
   // outputs, indexed by the caller's pair index
   int32_t* score;
@@ -49,6 +50,15 @@ struct WalkParams {
 
 constexpr uint32_t LAZY = 15;  // "came from S of the neighbour": resolved when the walk needs it
 
+template <class T>
+B2A_HD T ldg_ro(const T* p) {
+#if defined(__CUDA_ARCH__)
+  return __ldg(p);  // read-only path: K1 wrote it in an earlier launch
+#else
+  return *p;
+#endif
+}
+
 struct PairView {
   DevScoring sc;
   const int32_t* lut;
@@ -57,13 +67,14 @@ struct PairView {
   int32_t P;
   int32_t m, n, pi;
   int32_t G, R, TBW, nstrips, K;
-  const int4* bnd;     // [column][32]
+  const int4* bnd;     // [column][32]; bnd8: the same bytes as int2 records
   int32_t* rows;       // arrays of [rows_pad][32]
   int32_t rows_pad;
   uint16_t* rowm;      // [column][32]
   const uint32_t* tb;  // block base
   int32_t sub, g;      // task inside the block, slot inside the task
   int32_t packtrk;
+  int32_t bnd8 = 0;    // F_BND8 records (see load_bnd)
   int32_t maxn;        // block maximum of n
   int64_t bnd_base;    // boundary row of this pair: bnd[bnd_base + j * bnd_stride] (see bnd_index)
   int32_t bnd_stride;
@@ -95,12 +106,14 @@ struct PairView {
     return p == q ? sc.match_score : sc.mismatch_score;
   }
   B2A_HD int32_t& row(int arr, int32_t i) const { return rows[(arr * rows_pad + i) * 32 + pi]; }
+  // the record of column j as stored (decode_boundary); bnd8: the 8-byte record in x, y (z = w = 0)
   B2A_HD int4 load_bnd(int32_t j) const {
-#if defined(__CUDA_ARCH__)
-    return __ldg(&bnd[bnd_base + (int64_t)j * bnd_stride]);  // read-only path: K1 wrote it in an earlier launch
-#else
-    return bnd[bnd_base + (int64_t)j * bnd_stride];
-#endif
+    const int64_t k = bnd_base + (int64_t)j * bnd_stride;
+    if (bnd8) {
+      const int2 r = ldg_ro(&reinterpret_cast<const int2*>(bnd)[k]);
+      return make_int4(r.x, r.y, 0, 0);
+    }
+    return ldg_ro(&bnd[k]);
   }
   // compressed traceback nibble of an interior cell 1 <= i <= m-1, 1 <= j <= n
   B2A_HD uint32_t nib(int32_t i, int32_t j) const {
@@ -125,19 +138,21 @@ struct PairView {
 
 // Boundary row m-1 as K1 leaves it (scaled domain, b2a_fill.cuh): x = 4*S, y = 4*I + 2,
 // z/w = column tracker: packed key 4096*(max S) + (4095 - first row) [F_PACKTRK] or (4*(T), row).
+// bnd8 (F_BND8, always with F_PACKTRK): x = 4*S and 4*I + 2 as the low / high signed 16-bit halves, y = packed key.
 struct Boundary {
   int32_t S, I, Tv, Ti;
 };
-B2A_HD Boundary decode_boundary(const int4 b, const bool packtrk, const int32_t xs, const int32_t m) {
+B2A_HD Boundary decode_boundary(const int4 b, const bool packtrk, const bool bnd8, const int32_t xs, const int32_t m) {
   Boundary o;
-  o.S = b.x >> 2;
-  o.I = b.y >> 2;
+  o.S = (bnd8 ? lo_s16(b.x) : b.x) >> 2;
+  o.I = (bnd8 ? hi_s16(b.x) : b.y) >> 2;
   o.Tv = MIN_SCORE;
   o.Ti = m;
+  const int32_t key = bnd8 ? b.y : b.z;
   if (packtrk) {
-    if (b.z != (int32_t)0x80000000) {
-      o.Tv = (b.z >> 12) + xs;
-      o.Ti = 4095 - (b.z & 4095);
+    if (key != (int32_t)0x80000000) {
+      o.Tv = (key >> 12) + xs;
+      o.Ti = 4095 - (key & 4095);
     }
   } else if (b.z > -(1 << 29)) {
     o.Tv = b.z >> 2;
@@ -242,7 +257,7 @@ B2A_HD void finish_matrix_seq(const PairView& v, EndState& es) {
         Tv = MIN_SCORE;
         Ti = m;
       } else {
-        const Boundary b = decode_boundary(braw[u], v.packtrk != 0, xs, m);
+        const Boundary b = decode_boundary(braw[u], v.packtrk != 0, v.bnd8 != 0, xs, m);
         sup = b.S;
         iup = b.I;
         Tv = b.Tv;
@@ -582,7 +597,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
       int32_t lx;
       if (j == n) lx = LxN;
       else if (j == 0) lx = Lx0;
-      else lx = (m >= 2) ? m - decode_boundary(v.load_bnd(j), v.packtrk != 0, xs, m).Ti : 0;
+      else lx = (m >= 2) ? m - decode_boundary(v.load_bnd(j), v.packtrk != 0, v.bnd8 != 0, xs, m).Ti : 0;
       if (!filter_clips) {
         *(--ops_end) = 4;
         ++nops;
@@ -783,7 +798,7 @@ B2A_HD void finish_matrix_coop(const int lane, const PairView& v, EndState& es) 
     const int32_t jc = act ? j : n;  // idle lanes repeat the last column: loads stay in bounds, nothing is stored
     const int4 braw = braw_next;
     if (base + W <= n) braw_next = v.load_bnd(imin32(base + W + lane, n));
-    const Boundary b = decode_boundary(braw, pk, xs, m);
+    const Boundary b = decode_boundary(braw, pk, v.bnd8 != 0, xs, m);
     const int32_t q = v.ysym(jc);
     int32_t sdiag = C::up(b.S, 1);
     if (lane == 0) sdiag = cSup;
@@ -1109,6 +1124,7 @@ __device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& bl
   v.sub = lane / P;
   v.g = lane % P;
   v.packtrk = prm.packtrk;
+  v.bnd8 = prm.bnd8;
   v.maxn = (int32_t)blk.maxn;
   v.bnd_base = bnd_index(prm.G, 0, lane, v.maxn);
   v.bnd_stride = (int32_t)(bnd_index(prm.G, 1, lane, v.maxn) - v.bnd_base);
@@ -1162,6 +1178,7 @@ __device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& bl
   v.sub = pi / P;
   v.g = pi % P;
   v.packtrk = prm.packtrk;
+  v.bnd8 = prm.bnd8;
   v.maxn = (int32_t)blk.maxn;
   v.bnd_base = bnd_index(prm.G, 0, pi, v.maxn);
   v.bnd_stride = (int32_t)(bnd_index(prm.G, 1, pi, v.maxn) - v.bnd_base);
