@@ -90,7 +90,11 @@ typedef struct b2a_scoring {
   const int32_t* table;
   /* Symbols for which `table` is valid (e.g. "A-Z*" for bio::scores matrices).
    * NULL with a non-NULL table: the engine scans the batch for the symbols
-   * present (slower).  A sequence byte outside the alphabet is B2A_E_INVALID
+   * present (slower).  That scan is one flat pass over all of seq_blob, so
+   * bytes between sequences (padding) count as present: their table entries
+   * take part in the |score| <= 2^27 check and the score bound.  Pass the
+   * alphabet when such bytes have large or undefined entries.
+   * A sequence byte outside the alphabet is B2A_E_INVALID
    * (bio::scores::lookup would index out of bounds, scores/mod.rs:22-35). */
   const uint8_t* alphabet;
   uint32_t alphabet_len;

@@ -1531,17 +1531,9 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
   bp.num_cells = e->d_bcells.as<uint64_t>();
   bp.k4_status = e->d_bstatus.as<uint32_t>();
   bp.band_cols = e->d_bcols.as<uint32_t>();
-  // The strip-wavefront fill (b2a_banded_strip.cuh) covers every real score within +-2^26 (its sentinel
-  // arithmetic); row / column trackers only as packed keys (below).
-  {
-    const bool xs_dead = e->sc.xclip_suffix <= DEAD_CLIP, ys_dead = e->sc.yclip_suffix <= DEAD_CLIP;
-    const bool yp_live = e->sc.yclip_prefix > DEAD_CLIP;
-    // trackers are packed keys: every band cell's S has to be real (a live y-prefix clip guarantees it: S >=
-    // yclip_score(i)) and below 2^17; the column tracker's key also holds the row (x no longer than 4,095)
-    const bool trackers_ok = (xs_dead && ys_dead) || (yp_live && score_bound < (1ll << 17) && (xs_dead || maxm <= 4095));
-    bp.strip_ok = (e->banded_strip && e->banded_fast && score_bound < (1ll << 26) && trackers_ok) ? 1 : 0;
-    if (bp.strip_ok && e->banded_strip_lastcol) bp.strip_ok |= 2;  // bands that hold cells of column n as well
-  }
+  // The strip-wavefront fill (b2a_banded_strip.cuh) within its score range and tracker form (b2a_plan.h)
+  bp.strip_ok = (e->banded_strip && e->banded_fast && banded_strip_gate(e->sc, score_bound, maxm)) ? 1 : 0;
+  if (bp.strip_ok && e->banded_strip_lastcol) bp.strip_ok |= 2;  // bands that hold cells of column n as well
   e->strip_pairs = 0;
   bp.filter_clips = (mode == B2A_MODE_SEMIGLOBAL || mode == B2A_MODE_LOCAL) ? 1 : 0;
   bp.score = e->d_score.as<int32_t>();

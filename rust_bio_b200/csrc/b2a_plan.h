@@ -163,4 +163,16 @@ inline bool boundary8_ok(int flags, int64_t score_bound) {
   return (flags & F_PACKTRK) != 0 && 4 * score_bound + 3 < (1ll << 15);
 }
 
+// Whether the banded strip-wavefront fill (b2a_banded_strip.cuh) may take pairs of a batch; `sc` carries the mode's
+// clip preset.  Its sentinel arithmetic covers every real score within +-2^26.  Row / column trackers exist there
+// only as packed keys: every band cell's S has to be real (a live y-prefix clip guarantees it: S >= yclip_score(i))
+// and below 2^17, and the column tracker's key also holds the row (x no longer than 4,095).  Otherwise the pairs run
+// the K3 column loops.
+inline bool banded_strip_gate(const DevScoring& sc, int64_t score_bound, uint32_t maxm) {
+  const bool xs_dead = sc.xclip_suffix <= DEAD_CLIP, ys_dead = sc.yclip_suffix <= DEAD_CLIP;
+  const bool yp_live = sc.yclip_prefix > DEAD_CLIP;
+  const bool trackers_ok = (xs_dead && ys_dead) || (yp_live && score_bound < (1ll << 17) && (xs_dead || maxm <= 4095));
+  return score_bound < (1ll << 26) && trackers_ok;
+}
+
 }  // namespace b2a

@@ -752,7 +752,7 @@ extern "C" int sim_banded_warp32_one(int mode, const sim_scoring* s, uint32_t k,
 #include "../../rust_bio_b200/csrc/b2a_banded_strip.cuh"
 
 extern "C" int sim_banded_strip_task(int mode, const sim_scoring* s, uint32_t k, uint32_t w, const uint8_t* blob,
-                                     const uint64_t* x_off, const uint32_t* x_len, const uint64_t* y_off,
+                                     uint64_t blob_bytes, const uint64_t* x_off, const uint32_t* x_len, const uint64_t* y_off,
                                      const uint32_t* y_len, uint32_t n_pairs, uint32_t cap_matches, int garbage,
                                      int32_t* score, uint32_t* coords /*4 per pair*/, uint32_t* n_ops,
                                      uint32_t* clip_len, uint32_t* status, uint32_t* path, uint8_t* ops,
@@ -772,19 +772,24 @@ extern "C" int sim_banded_strip_task(int mode, const sim_scoring* s, uint32_t k,
   sc.mismatch_score = s->mismatch_score;
   const int32_t* table = s->table;
   auto run32 = [&](std::function<void(int)> body) { LaneFibers::run(body); };
-  // tabulated MatchFunc: codes over the bytes present and K1's scaled LUT, as the engine's stage_front builds them
-  std::vector<uint8_t> cmap(256, 0xFF);
-  std::vector<int32_t> lut_scaled;
-  if (table) {
+  // the alphabet as the engine's stage_front finds it: the caller's, else every byte value of the blob in one flat pass
+  // (the padding between sequences included)
+  std::vector<int> syms;
+  {
     std::vector<bool> present(256, false);
-    for (uint32_t p = 0; p < n_pairs; ++p) {
-      for (uint32_t t = 0; t < x_len[p]; ++t) present[blob[x_off[p] + t]] = true;
-      for (uint32_t t = 0; t < y_len[p]; ++t) present[blob[y_off[p] + t]] = true;
+    if (s->alphabet && s->alphabet_len) {
+      for (uint32_t q = 0; q < s->alphabet_len; ++q) present[s->alphabet[q]] = true;
+    } else {
+      for (uint64_t t = 0; t < blob_bytes; ++t) present[blob[t]] = true;
     }
-    std::vector<int> syms;
     for (int b = 0; b < 256; ++b)
       if (present[b]) syms.push_back(b);
     if (syms.empty()) syms.push_back(0);
+  }
+  // tabulated MatchFunc: codes over that alphabet and K1's scaled LUT, as stage_front builds them
+  std::vector<uint8_t> cmap(256, 0xFF);
+  std::vector<int32_t> lut_scaled;
+  if (table) {
     if (syms.size() > 128) return -3;
     sc.alpha = (int32_t)syms.size();
     for (int a = 0; a < sc.alpha; ++a) cmap[syms[a]] = (uint8_t)a;
@@ -793,11 +798,22 @@ extern "C" int sim_banded_strip_task(int mode, const sim_scoring* s, uint32_t k,
       for (int b = 0; b < sc.alpha; ++b)
         lut_scaled[(size_t)a * sc.alpha + b] = 4 * table[(size_t)syms[a] * 256 + syms[b]] + 3 - (4 * sc.gap_open + 1);
   }
-  // the host's part of the decision (b2a_engine.cu banded_impl)
-  const bool xs_dead = sc.xclip_suffix <= DEAD_CLIP, ys_dead = sc.yclip_suffix <= DEAD_CLIP, yp_live = sc.yclip_prefix > DEAD_CLIP;
-  uint32_t maxm = 0;
-  for (uint32_t p = 0; p < n_pairs; ++p) maxm = std::max(maxm, x_len[p]);
-  const bool batch_ok = (xs_dead && ys_dead) || (yp_live && (xs_dead || maxm <= 4095));
+  // the host's part of the decision (b2a_engine.cu banded_impl): score_bound as stage_front computes it (the largest
+  // |score| over that alphabet), then the gate of b2a_plan.h
+  uint32_t maxm = 0, maxn = 0;
+  for (uint32_t p = 0; p < n_pairs; ++p) {
+    maxm = std::max(maxm, x_len[p]);
+    maxn = std::max(maxn, y_len[p]);
+  }
+  int64_t maxabs = std::max<int64_t>(std::llabs((long long)s->match_score), std::llabs((long long)s->mismatch_score));
+  if (table) {
+    maxabs = 0;
+    for (int a : syms)
+      for (int b : syms) maxabs = std::max<int64_t>(maxabs, std::llabs((long long)table[(size_t)a * 256 + b]));
+  }
+  const int64_t unit = std::max<int64_t>(maxabs, std::max<int64_t>(-(int64_t)sc.gap_open, -(int64_t)sc.gap_extend));
+  const int64_t score_bound = ((int64_t)maxm + maxn + 2) * unit - (int64_t)sc.gap_open;
+  const bool batch_ok = banded_strip_gate(sc, score_bound, maxm);
   std::vector<std::vector<uint32_t>> rngs(n_pairs);
   std::vector<uint64_t> cells(n_pairs, 0);
   std::vector<uint32_t> cols(3 * (size_t)n_pairs + 3, 0), k4(n_pairs, 0), elig;
@@ -967,4 +983,16 @@ extern "C" int sim_scoring_flags(int32_t xclip_prefix, int32_t xclip_suffix, int
   sc.yclip_suffix = yclip_suffix;
   sc.alpha = alpha;
   return scoring_flags(sc, score_bound, maxm, maxn);
+}
+
+// whether the engine lets a banded batch run the strip-wavefront fill (b2a_plan.h banded_strip_gate); clips with the
+// mode's preset applied
+extern "C" int sim_banded_strip_gate(int32_t xclip_prefix, int32_t xclip_suffix, int32_t yclip_prefix,
+                                     int32_t yclip_suffix, int64_t score_bound, uint32_t maxm) {
+  DevScoring sc{};
+  sc.xclip_prefix = xclip_prefix;
+  sc.xclip_suffix = xclip_suffix;
+  sc.yclip_prefix = yclip_prefix;
+  sc.yclip_suffix = yclip_suffix;
+  return banded_strip_gate(sc, score_bound, maxm) ? 1 : 0;
 }

@@ -228,7 +228,8 @@ def banded_strip_task(mode, orc_scoring, k, w, pairs, cap_matches=4096):
         path = np.zeros(n, dtype=np.uint32)
         L = lib()
         L.sim_banded_strip_task.restype = C.c_int
-        rc = L.sim_banded_strip_task(int(mode), C.byref(s), C.c_uint32(k), C.c_uint32(w), p(blob), p(x_off), p(x_len),
+        rc = L.sim_banded_strip_task(int(mode), C.byref(s), C.c_uint32(k), C.c_uint32(w), p(blob),
+                                     C.c_uint64(len(blob)), p(x_off), p(x_len),
                                      p(y_off), p(y_len), C.c_uint32(n), C.c_uint32(cap_matches), int(garbage), p(score),
                                      p(coords), p(n_ops), p(clip), p(status), p(path), p(ops), p(ops_off))
         assert rc == 0, rc
