@@ -190,6 +190,23 @@ int32_t b2a_engine_set_pipeline(b2a_engine* e, int32_t chunks);
 int32_t b2a_align_batch(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
                         const b2a_pairs* pairs, b2a_results* results, b2a_stats* stats);
 
+/* Aligner::{custom,global,semiglobal,local} reduced to Alignment.score / xend / yend: no traceback is stored or walked.
+ * For each pair, score, xend and yend are what b2a_align_batch returns; xstart, ystart and the ops are not computed
+ * (they come out of the prefix end of the traceback walk).  The fill keeps no traceback, so waves close on the rest of
+ * the per-wave scratch (boundary rows, row trackers, row m) against the traceback budget, and K2 walks only along
+ * row m and column n: once the walk enters a cell with i < m and j < n, xend and yend are final.
+ *   stage_scores: as b2a_batch_stage; b2a_batch_run then runs the score-only batch.
+ *   b2a_batch_fetch on it fills score, xend, yend and status; xstart, ystart, ops, ops_off and clip_len must be NULL
+ *   (else B2A_E_INVALID).  b2a_batch_records*, b2a_batch_compact* and b2a_gathered_fetch return B2A_E_STATE.
+ *   b2a_align_batch_scores is single-shot at every size (no chunk pipeline).
+ * A forced fill shape (b2a_engine_set_tuning) other than 1x16, 8x16, 8x20, 32x8 or 32x16 is B2A_E_UNSUPPORTED.
+ * status: a pair whose walk would panic or never end while still on row m / column n is B2A_PAIR_PANIC, as with
+ * b2a_align_batch.  A panic only the interior walk would meet (mod.rs:905) cannot be seen without the traceback:
+ * such a pair reports its score. */
+int32_t b2a_batch_stage_scores(b2a_engine* e, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs);
+int32_t b2a_align_batch_scores(b2a_engine* e, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
+                               b2a_results* results, b2a_stats* stats);
+
 /* Packed input (SURVEY 8f rank 2): the sequences as bio::data_structures::bitenc::BitEnc storage
  * (src/data_structures/bitenc.rs:50-56: 32-bit blocks, `width` bits per symbol, 32 - 32 % width usable bits per
  * block; symbol i sits at bit (i*width) % usable of block (i*width) / usable, bitenc.rs:319-338), holding the ranks

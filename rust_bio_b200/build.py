@@ -19,6 +19,8 @@ VARIANT = os.environ.get("B2A_VARIANT", "")  # dev knob: a differently configure
 OBJ = os.path.join(CSRC, "build" + (("_" + VARIANT) if VARIANT else ""))
 SO = os.path.join(CSRC, "libb200align%s.so" % (("_" + VARIANT) if VARIANT else ""))
 SHAPES = [(1, 16), (1, 8), (1, 20), (2, 16), (2, 20), (4, 16), (8, 16), (8, 20), (32, 8), (32, 16)]
+# the shapes the engine's automatic choice picks also get the score-only (F_NOTB) fill, in translation units of their own
+NOTB_SHAPES = [(1, 16), (8, 16), (8, 20), (32, 8), (32, 16)]
 # minimum resident CTAs per SM asked of ptxas per shape (__launch_bounds__): measured choice, see DESIGN.md
 MIN_BLOCKS = {(1, 16): int(os.environ.get("B2A_MINB_1_16", "3")), (8, 16): int(os.environ.get("B2A_MINB_8_16", "3")),
               (8, 20): int(os.environ.get("B2A_MINB_8_20", "1"))}  # 8x20 at 3 CTAs/SM (168 registers) was slower
@@ -58,12 +60,14 @@ def build(force: bool = False, verbose: bool = False) -> str:
     hdrs = [os.path.join(CSRC, h) for h in HEADERS]
     jobs = []
     objs = []
-    for g, r in SHAPES:
-        o = os.path.join(OBJ, f"fill_{g}_{r}.o")
-        objs.append(o)
-        src = os.path.join(CSRC, "b2a_fill_inst.cu")
-        if force or _stale(o, hdrs + [src]):
-            jobs.append([NVCC, *FLAGS, f"-DB2A_G={g}", f"-DB2A_R={r}", f"-DB2A_MINB={MIN_BLOCKS.get((g, r), 1)}", "-c", src, "-o", o])
+    src = os.path.join(CSRC, "b2a_fill_inst.cu")
+    for notb, shapes in ((False, SHAPES), (True, NOTB_SHAPES)):
+        for g, r in shapes:
+            o = os.path.join(OBJ, f"fill_{'notb_' if notb else ''}{g}_{r}.o")
+            objs.append(o)
+            if force or _stale(o, hdrs + [src]):
+                jobs.append([NVCC, *FLAGS, f"-DB2A_G={g}", f"-DB2A_R={r}", f"-DB2A_MINB={MIN_BLOCKS.get((g, r), 1)}",
+                             *(["-DB2A_NOTB"] if notb else []), "-c", src, "-o", o])
     eo = os.path.join(OBJ, "engine.o")
     objs.append(eo)
     esrc = os.path.join(CSRC, "b2a_engine.cu")

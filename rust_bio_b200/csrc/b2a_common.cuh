@@ -84,6 +84,8 @@ enum : int {
   F_BND8 = 256,      // with F_PACKTRK: the strip boundary record is 8 bytes, int2 {(I4 << 16) | (S4 & 0xffff), packed
                      // column-tracker key}, instead of int4 {S4, I4, key, row}.  Needs every S4 = 4*S and I4 = 4*I + 2
                      // to fit a signed 16-bit half: 4*score_bound + 3 < 2^15 (boundary8_ok in b2a_plan.h)
+  F_NOTB = 512,      // score-only batches: no interior traceback is accumulated or stored (the last column still writes
+                     // its nibbles to ROWS_NL: K2's fix-ups and the edge walk read them)
 };
 #ifndef B2A_KREL_BITS
 #define B2A_KREL_BITS 12  // (a test build shortens the chunks to exercise the flushes on small inputs)

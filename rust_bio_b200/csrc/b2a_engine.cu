@@ -57,9 +57,16 @@ struct DevBuf {
 };
 
 const FillLaunch kFillShapes[] = {
-    {1, 16, launch_fill_1_16}, {1, 8, launch_fill_1_8},   {1, 20, launch_fill_1_20},
-    {2, 16, launch_fill_2_16}, {2, 20, launch_fill_2_20}, {4, 16, launch_fill_4_16},
-    {8, 16, launch_fill_8_16}, {8, 20, launch_fill_8_20}, {32, 8, launch_fill_32_8}, {32, 16, launch_fill_32_16},
+    {1, 16, launch_fill_1_16, launch_fill_notb_1_16},
+    {1, 8, launch_fill_1_8, nullptr},
+    {1, 20, launch_fill_1_20, nullptr},
+    {2, 16, launch_fill_2_16, nullptr},
+    {2, 20, launch_fill_2_20, nullptr},
+    {4, 16, launch_fill_4_16, nullptr},
+    {8, 16, launch_fill_8_16, launch_fill_notb_8_16},
+    {8, 20, launch_fill_8_20, launch_fill_notb_8_20},
+    {32, 8, launch_fill_32_8, launch_fill_notb_32_8},
+    {32, 16, launch_fill_32_16, launch_fill_notb_32_16},
 };
 
 const FillLaunch* find_shape(int G, int R) {
@@ -121,6 +128,7 @@ struct b2a_engine {
 
   // batch state
   bool staged = false, ran = false;
+  bool score_only = false;  // staged by b2a_batch_stage_scores: F_NOTB fill, score-only K2, no ops compaction
   Plan plan;
   DevScoring sc{};
   int flags = 0, mode = 0;
@@ -387,6 +395,7 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
                            uint32_t& maxm, uint32_t& maxn, int64_t& score_bound) {
   if (!e || !s || !pairs) return B2A_E_INVALID;
   e->staged = e->ran = false;
+  e->score_only = false;
   if (mode < 0 || mode > 3) return e->fail(B2A_E_INVALID, "mode must be B2A_MODE_*");
   int rc = validate_scoring(e, s);
   if (rc) return rc;
@@ -583,12 +592,15 @@ static int32_t compact_ops(b2a_engine* e, uint64_t scratch_bytes, cudaStream_t s
 
 extern "C" {
 
-int32_t b2a_batch_stage(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs) {
+// score_only: the batch of b2a_batch_stage_scores -- the fill's F_NOTB twin and a plan without traceback bytes
+static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs,
+                                bool score_only) {
   if (!e || !s || !pairs) return B2A_E_INVALID;
   uint32_t maxm = 0, maxn = 0;
   int64_t score_bound = 0;
   int rc = stage_front(e, mode, s, pairs, maxm, maxn, score_bound);
   if (rc) return rc;
+  if (score_only) e->flags |= F_NOTB;
   const uint64_t n = e->n_pairs;
   const DevScoring sc = e->sc;
   cudaStream_t st = e->stream;
@@ -621,6 +633,9 @@ int32_t b2a_batch_stage(b2a_engine* e, int32_t mode, const b2a_scoring* s, const
     const uint64_t pad16 = (rows + 511) / 512 * 512, pad8 = (rows + 255) / 256 * 256;
     R = (pad16 * 100 <= pad8 * 112) ? 16 : 8;
   }
+  if (score_only && !e->shape->launch_notb)
+    return e->fail(B2A_E_UNSUPPORTED, "score-only batches run only the fill shapes the automatic choice picks (1x16, 8x16, "
+                                      "8x20, 32x8, 32x16); the forced shape has no score-only fill kernel");
   const Plan& pl = e->plan;
 
   // device memory
@@ -690,8 +705,17 @@ int32_t b2a_batch_stage(b2a_engine* e, int32_t mode, const b2a_scoring* s, const
   // the caller's arrays are read by the copies above: wait for them unless the caller (the chunk pipeline of
   // b2a_align_batch) keeps them alive itself
   if (!e->stage_nosync) CK(cudaStreamSynchronize(st));
+  e->score_only = score_only;
   e->staged = true;
   return B2A_OK;
+}
+
+int32_t b2a_batch_stage(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs) {
+  return batch_stage_impl(e, mode, s, pairs, false);
+}
+
+int32_t b2a_batch_stage_scores(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs) {
+  return batch_stage_impl(e, mode, s, pairs, true);
 }
 
 int32_t b2a_batch_run(b2a_engine* e) {
@@ -700,6 +724,10 @@ int32_t b2a_batch_run(b2a_engine* e) {
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const Plan& pl = e->plan;
   cudaStream_t st = e->stream;
+  // a score-only batch: the F_NOTB fill (no traceback) and the K2 that stops where xend / yend are final
+  const FillLaunchFn fill = e->score_only ? e->shape->launch_notb : e->shape->launch;
+  void (*const walk_warp_k)(const WalkParams) = e->score_only ? walk_warp_kernel<true> : walk_warp_kernel<false>;
+  void (*const walk_lane_k)(const WalkParams) = e->score_only ? walk_kernel<true> : walk_kernel<false>;
   // pipeline slots put K2 and what follows on their high-priority stream (several waves share scratch: one stream)
   const bool use_tail = e->is_slot && e->tail_stream != nullptr && pl.waves.size() == 1;
   e->tail_used = use_tail;
@@ -737,7 +765,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     fp.seq = e->d_seq.as<uint8_t>();
     fp.bnd = e->d_bnd.as<uint8_t>();
     fp.rows = e->d_rows.as<uint8_t>();
-    fp.tb = e->d_tb.as<uint8_t>();
+    fp.tb = e->score_only ? nullptr : e->d_tb.as<uint8_t>();
     fp.lut = e->d_lut.as<int32_t>() + (size_t)e->sc.alpha * e->sc.alpha;  // the scaled copy
     fp.task_counter = ctl + 2 + wi;
     fp.smem_seq_bytes = pl.smem_seq_bytes;
@@ -804,7 +832,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
       if (!wcta_warps) wcta_warps = (uint64_t)per_warp * 8 <= 96 * 1024 ? 8u : 4u;
       per_warp_smem = (uint64_t)per_warp * wcta_warps <= 96 * 1024 ? per_warp : 0u;
       if ((size_t)per_warp_smem * wcta_warps > 48 * 1024)
-        CK(cudaFuncSetAttribute(walk_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp_smem * wcta_warps)));
+        CK(cudaFuncSetAttribute(walk_warp_k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(per_warp_smem * wcta_warps)));
     }
     if (!wcta_warps) wcta_warps = 4;
     wp.seq_smem_per_warp = per_warp_smem;
@@ -825,7 +853,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     if (e->tail_split && !overlap && pl.waves.size() == 1 && warp_walk && pl.G != 32 && !use_tail && e->walk_mode != 1 &&
         fp.task_limit == 0) {
       int resident = 0;
-      CK(e->shape->launch(e->flags, fp, fill_tasks, e->num_sms, st, &resident, 1));
+      CK(fill(e->flags, fp, fill_tasks, e->num_sms, st, &resident, 1));
       const uint32_t slots = (uint32_t)resident, tasks = fill_tasks;
       if (slots > 0 && tasks > slots) {
         const uint32_t rounds = tasks / slots, rem = tasks % slots;
@@ -860,7 +888,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
       if (e->split_timing && !e->split_ev[0])
         for (auto& v : e->split_ev) CK(cudaEventCreate(&v));
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[0], st));
-      CK(e->shape->launch(e->flags, fa, fa.nblocks * (uint32_t)pl.G, e->num_sms, st, &e->last_grid, 0));
+      CK(fill(e->flags, fa, fa.nblocks * (uint32_t)pl.G, e->num_sms, st, &e->last_grid, 0));
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[1], st));
       CK(cudaEventRecord(e->sub_ev[0], st));  // fill A done
       // fill B + walk B on the high-priority stream, walk A on the auxiliary one
@@ -868,13 +896,13 @@ int32_t b2a_batch_run(b2a_engine* e) {
       cudaStream_t sB = e->tail_stream, sA = e->aux_stream;
       CK(cudaStreamWaitEvent(sB, e->sub_ev[0], 0));
       CK(cudaStreamWaitEvent(sA, e->sub_ev[0], 0));
-      CK(e->shape->launch(e->flags, fb, fb.nblocks * (uint32_t)pl.G, e->num_sms, sB, nullptr, 0));
+      CK(fill(e->flags, fb, fb.nblocks * (uint32_t)pl.G, e->num_sms, sB, nullptr, 0));
       CK(cudaEventRecord(e->wave_ev[3 * wi + 1], sB));  // every fill has finished
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[2], sB));
-      walk_warp_kernel<<<wa.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, sA>>>(wa);
+      walk_warp_k<<<wa.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, sA>>>(wa);
       CK(cudaGetLastError());
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[3], sA));
-      walk_warp_kernel<<<wb.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, sB>>>(wb);
+      walk_warp_k<<<wb.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, sB>>>(wb);
       CK(cudaGetLastError());
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[4], sB));
       e->split_ran = true;
@@ -915,7 +943,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
         f2.nblocks = hi_b - lo_b;
         f2.task_counter = ctl + 8 + sidx;
         f2.task_limit = 1;  // CTAs retire after one task per warp: the walks' CTAs get onto the SMs in between
-        CK(e->shape->launch(e->flags, f2, f2.nblocks * (uint32_t)pl.G, e->num_sms, fs, &e->last_grid, 0));
+        CK(fill(e->flags, f2, f2.nblocks * (uint32_t)pl.G, e->num_sms, fs, &e->last_grid, 0));
         ++e->launches;
         CK(cudaEventRecord(e->sub_ev[sidx], fs));
         CK(cudaStreamWaitEvent(e->tail_stream, e->sub_ev[sidx], 0));
@@ -923,8 +951,8 @@ int32_t b2a_batch_run(b2a_engine* e) {
         WalkParams w2 = wp;
         w2.blocks = wp.blocks + lo_b;
         w2.nblocks = hi_b - lo_b;
-        if (warp_walk) walk_warp_kernel<<<w2.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, e->tail_stream>>>(w2);
-        else walk_kernel<<<(w2.nblocks * 32 + 127) / 128, 128, 0, e->tail_stream>>>(w2);
+        if (warp_walk) walk_warp_k<<<w2.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, e->tail_stream>>>(w2);
+        else walk_lane_k<<<(w2.nblocks * 32 + 127) / 128, 128, 0, e->tail_stream>>>(w2);
         CK(cudaGetLastError());
         ++e->launches;
       }
@@ -936,7 +964,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
       continue;
     }
     CK(cudaEventRecord(e->wave_ev[3 * wi + 0], st));
-    CK(e->shape->launch(e->flags, fp, fill_tasks, e->num_sms, st, &e->last_grid, 0));
+    CK(fill(e->flags, fp, fill_tasks, e->num_sms, st, &e->last_grid, 0));
     ++e->launches;
     CK(cudaEventRecord(e->wave_ev[3 * wi + 1], st));
     if (use_tail) {  // K2 and everything after it on the high-priority stream
@@ -949,10 +977,10 @@ int32_t b2a_batch_run(b2a_engine* e) {
       // pairs share every cache line); one WARP per pair cuts the per-pair latency chain (prefix-maximum passes,
       // prefetched walk) and is what small / medium batches and long sequences need (b2a_walk.cuh).
       if (warp_walk) {
-        walk_warp_kernel<<<nb * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, st>>>(wp);  // 32 warps (pairs) per block of the plan
+        walk_warp_k<<<nb * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, st>>>(wp);  // 32 warps (pairs) per block of the plan
       } else {
         const unsigned wgrid = (nb * 32 + 127) / 128;
-        walk_kernel<<<wgrid, 128, 0, st>>>(wp);
+        walk_lane_k<<<wgrid, 128, 0, st>>>(wp);
       }
       CK(cudaGetLastError());
       ++e->launches;
@@ -962,7 +990,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     ++wi;
   }
   CK(cudaEventRecord(e->ev[4], st));
-  {
+  if (!e->score_only) {
     int rc2 = compact_ops(e, pl.ops_bytes, st);
     if (rc2) return rc2;
   }
@@ -974,6 +1002,9 @@ int32_t b2a_batch_run(b2a_engine* e) {
 int32_t b2a_batch_fetch(b2a_engine* e, b2a_results* r, b2a_stats* stats) {
   if (!e) return B2A_E_INVALID;
   if (!e->ran) return e->fail(B2A_E_STATE, "b2a_batch_fetch before b2a_batch_run");
+  if (e->score_only && r && (r->xstart || r->ystart || r->ops || r->ops_off || r->clip_len))
+    return e->fail(B2A_E_INVALID, "a score-only batch has only score, xend, yend and status: xstart, ystart, ops, "
+                                  "ops_off and clip_len must be NULL");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   cudaStream_t st = e->res_stream();
   const uint64_t n = e->n_pairs;
@@ -994,7 +1025,9 @@ int32_t b2a_batch_fetch(b2a_engine* e, b2a_results* r, b2a_stats* stats) {
     CK(down(r->clip_len, e->d_clip, n * 16));
     CK(down(r->status, e->d_status, n * 4));
     uint64_t total = 0;
-    if (r->ops_off) {
+    if (e->score_only) {
+      // no ops were made
+    } else if (r->ops_off) {
       CK(down(r->ops_off, e->d_opsoff, (n + 1) * 8));
       CK(cudaStreamSynchronize(st));
       total = r->ops_off[n];
@@ -1326,10 +1359,22 @@ int32_t b2a_align_batch(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
   // large batches with host outputs: pipeline chunks so copies and planning overlap the kernels
   if (e->pipe_chunks >= 2 && results && pairs->n_pairs >= 262144) {
     e->staged = e->ran = false;
+    e->score_only = false;
     if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
     return align_batch_pipelined(e, mode, scoring, pairs, results, stats);
   }
   int rc = b2a_batch_stage(e, mode, scoring, pairs);
+  if (rc) return rc;
+  rc = b2a_batch_run(e);
+  if (rc) return rc;
+  return b2a_batch_fetch(e, results, stats);
+}
+
+// single-shot at every size: the score-only path has no chunk pipeline
+int32_t b2a_align_batch_scores(b2a_engine* e, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
+                               b2a_results* results, b2a_stats* stats) {
+  if (!e || !scoring || !pairs) return B2A_E_INVALID;
+  int rc = b2a_batch_stage_scores(e, mode, scoring, pairs);
   if (rc) return rc;
   rc = b2a_batch_run(e);
   if (rc) return rc;
@@ -1816,6 +1861,7 @@ uint32_t b2a_record_stride(uint32_t max_m, uint32_t max_n) {
 int32_t b2a_batch_records_into(b2a_engine* e, void* dev_dst, uint64_t dst_bytes, uint32_t* stride_bytes) {
   if (!e) return B2A_E_INVALID;
   if (!e->ran) return e->fail(B2A_E_STATE, "records requested before b2a_batch_run");
+  if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to put in records");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint32_t stride = b2a_record_stride(e->plan.maxm, e->plan.maxn);
   if (stride_bytes) *stride_bytes = stride;
@@ -1836,6 +1882,7 @@ int32_t b2a_batch_records_into(b2a_engine* e, void* dev_dst, uint64_t dst_bytes,
 int32_t b2a_batch_records(b2a_engine* e, void** dev_records, uint32_t* stride_bytes, uint64_t* n_records) {
   if (!e || !dev_records) return B2A_E_INVALID;
   if (!e->ran) return e->fail(B2A_E_STATE, "records requested before b2a_batch_run");
+  if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to put in records");
   const uint32_t stride = b2a_record_stride(e->plan.maxm, e->plan.maxn);
   CK(e->d_records.reserve(e->n_pairs * (uint64_t)stride + 16));
   int rc = b2a_batch_records_into(e, e->d_records.p, e->n_pairs * (uint64_t)stride, stride_bytes);
@@ -1848,6 +1895,7 @@ int32_t b2a_batch_records(b2a_engine* e, void** dev_records, uint32_t* stride_by
 int32_t b2a_batch_compact_bytes(b2a_engine* e, uint64_t* segment_bytes) {
   if (!e || !segment_bytes) return B2A_E_INVALID;
   if (!e->ran) return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run");
+  if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to compact");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = e->n_pairs;
   uint64_t total = 0;
@@ -1862,6 +1910,7 @@ int32_t b2a_batch_compact_bytes(b2a_engine* e, uint64_t* segment_bytes) {
 int32_t b2a_batch_compact_into(b2a_engine* e, void* dev_dst, uint64_t dst_bytes) {
   if (!e || !dev_dst) return B2A_E_INVALID;
   if (!e->ran) return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run");
+  if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to compact");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = e->n_pairs;
   if (e->compact_hdr[0] != n) return e->fail(B2A_E_STATE, "b2a_batch_compact_bytes must be called first");
@@ -1896,6 +1945,7 @@ __global__ void compact_header_kernel(uint64_t* hdr, const uint64_t* ops_off, ui
 int32_t b2a_batch_compact_fixed(b2a_engine* e, void* dev_dst, uint64_t capacity_bytes) {
   if (!e || !dev_dst) return B2A_E_INVALID;
   if (!e->ran) return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run");
+  if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to compact");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = e->n_pairs;
   if (capacity_bytes < 64 + 40 * n) return e->fail(B2A_E_CAPACITY, "compact segment capacity below 64 + 40 n_pairs");
@@ -1920,6 +1970,7 @@ int32_t b2a_batch_compact_fixed(b2a_engine* e, void* dev_dst, uint64_t capacity_
 int32_t b2a_gathered_fetch(b2a_engine* e, const void* dev_gathered, uint64_t segment_bytes, uint32_t n_segments,
                            b2a_results* r, uint64_t* n_pairs_total, uint64_t* d2h_bytes) {
   if (!e || !dev_gathered || !r || segment_bytes < 64) return B2A_E_INVALID;
+  if (e->score_only) return e->fail(B2A_E_STATE, "the engine holds a score-only batch: gathered segments are full results");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   cudaStream_t st = e->stream;
   const uint8_t* base = reinterpret_cast<const uint8_t*>(dev_gathered);

@@ -210,6 +210,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
   constexpr bool PR = (FLAGS & F_PACKREL) != 0;  // packed keys with relative indices (see F_PACKREL): here like PK,
   constexpr bool PK = (FLAGS & F_PACKTRK) != 0 || PR;  // the caller passes chunk- / strip-relative cj and rowbase
   constexpr bool RELU = (FLAGS & F_RELU) != 0;
+  constexpr bool NOTB = (FLAGS & F_NOTB) != 0;
   constexpr bool TMASK = MASKED && !LUT;  // the column tracker has to skip the padded rows explicitly
   // S travels between cells as "S + open": So_d = S4 + go4d feeds the D chain of the next column and (as
   // the diagonal input) M of the next column, whose LUT/compare scores are pre-biased by -go4d; the I chain
@@ -254,8 +255,8 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
     // nibble = code | iext << 2 | dext << 3 = (sP - s4) + min(i4 - iop, 4) + 2 * min(d4 - dop, 4),
     // accumulated as tbacc*16 + nibble (the oldest nibble falls off the top)
     const int32_t fi = addmin(i4, -iop, 4), fd = addmin(d4, -dop, 4);
-    const int32_t nib = fmad(fd, k2, fi) + sP - s4;
-    tbacc[r] = (uint32_t)(fmad((int32_t)tbacc[r], k16, fmad(fd, k2, fi)) + sP - s4);
+    const int32_t nib = fmad(fd, k2, fi) + sP - s4;  // (NOTB: needed by the LAST column only, dead elsewhere)
+    if (!NOTB) tbacc[r] = (uint32_t)(fmad((int32_t)tbacc[r], k16, fmad(fd, k2, fi)) + sP - s4);
     if (TC) {
       if (PK) {
         if (TMASK) {
@@ -318,6 +319,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
   constexpr bool PR = (FLAGS & F_PACKREL) != 0;
   constexpr bool PK = (FLAGS & F_PACKTRK) != 0 || PR;  // packed keys in the lanes (PR: relative indices)
   constexpr bool B8 = (FLAGS & F_BND8) != 0;           // 8-byte boundary record (with F_PACKTRK only)
+  constexpr bool NOTB = (FLAGS & F_NOTB) != 0;         // score-only: no traceback words (c.tb may be null)
   static_assert(!B8 || ((FLAGS & F_PACKTRK) != 0 && !PR), "F_BND8 needs the packed column tracker with absolute rows");
   constexpr int P = 32 / G;
   constexpr int TBW = tbw_of(R);
@@ -416,7 +418,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       MASKED ? (rv >= 1 && (c.l == G - 1 || rowbase + R >= m - 1)) : (c.l == G - 1);
   int32_t cap_s = 0, cap_i = 0;
   uint32_t yw = 0;
-  uint4* tbs = c.tb + (size_t)s * c.K * TBW * 32;
+  uint4* tbs = NOTB ? nullptr : c.tb + (size_t)s * c.K * TBW * 32;
   const int32_t nsteps = c.K * 8;
 
   if (PR && TR) {
@@ -528,7 +530,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       in_i = iup;
       in_tv = Tv;
       in_ti = Ti;
-    } else {
+    } else if (!NOTB) {
 #pragma unroll
       for (int r = 0; r < R; ++r) tbacc[r] <<= 4;
     }
@@ -544,7 +546,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
         }
       }
     }
-    if ((t & 7) == 7) {
+    if (!NOTB && (t & 7) == 7) {
       uint4* dst = tbs + (size_t)(t >> 3) * TBW * 32 + c.lane;
 #pragma unroll
       for (int qd = 0; qd < TBW; ++qd) {
@@ -736,8 +738,8 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
     c.uniform = blk.uniform != 0;
     c.bnd = reinterpret_cast<int4*>(prm.bnd + blk.bnd_off);
     c.rows = reinterpret_cast<int32_t*>(prm.rows + blk.rows_off);
-    c.tb = reinterpret_cast<uint4*>(prm.tb + blk.tb_off) +
-           (size_t)sub * blk.nstrips * blk.K * TBW * 32;
+    c.tb = (FLAGS & F_NOTB) ? nullptr
+                            : reinterpret_cast<uint4*>(prm.tb + blk.tb_off) + (size_t)sub * blk.nstrips * blk.K * TBW * 32;
     while (!mbar_try_wait(bar, parity)) {
     }
     parity ^= 1u;

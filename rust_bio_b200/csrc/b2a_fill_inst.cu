@@ -1,8 +1,16 @@
-// One (G, R) shape of the K1 fill kernel: compile with -DB2A_G=<G> -DB2A_R=<R>.
+// One (G, R) shape of the K1 fill kernel: compile with -DB2A_G=<G> -DB2A_R=<R>.  With -DB2A_NOTB the same
+// flag cases are instantiated with F_NOTB added (score-only batches) as launch_fill_notb_<G>_<R>, in a
+// translation unit of their own so that the build stays parallel.
 #include "b2a_fill_launch.h"
 
 #ifndef B2A_G
 #error "compile with -DB2A_G=... -DB2A_R=..."
+#endif
+
+#ifdef B2A_NOTB
+#define B2A_LAUNCH_NAME launch_fill_notb_
+#else
+#define B2A_LAUNCH_NAME launch_fill_
 #endif
 
 namespace b2a {
@@ -42,11 +50,16 @@ cudaError_t go(const FillParams& prm, uint32_t ntasks, int num_sms, cudaStream_t
 #define B2A_CAT2(a, b, c) a##b##_##c
 #define B2A_CAT(a, b, c) B2A_CAT2(a, b, c)
 
-cudaError_t B2A_CAT(launch_fill_, B2A_G, B2A_R)(int flags, const FillParams& prm, uint32_t ntasks,
-                                                int num_sms, cudaStream_t stream, int* grid_out, int dry) {
+cudaError_t B2A_CAT(B2A_LAUNCH_NAME, B2A_G, B2A_R)(int flags, const FillParams& prm, uint32_t ntasks,
+                                                   int num_sms, cudaStream_t stream, int* grid_out, int dry) {
   constexpr int ALL = F_TRACK_ROWS | F_TRACK_COLS | F_CLIPX;
+#ifdef B2A_NOTB
+  constexpr int NOTB = F_NOTB;
+#else
+  constexpr int NOTB = 0;
+#endif
 #define B2A_CASE(F) \
-  case (F): return go<(F)>(prm, ntasks, num_sms, stream, grid_out, dry);
+  case (NOTB | (F)): return go<(NOTB | (F))>(prm, ntasks, num_sms, stream, grid_out, dry);
   switch (flags) {
     B2A_CASE(0)
     B2A_CASE(F_TRACK_ROWS)

@@ -7,17 +7,24 @@
 
 namespace b2a {
 
+typedef cudaError_t (*FillLaunchFn)(int flags, const FillParams& prm, uint32_t ntasks, int num_sms,
+                                    cudaStream_t stream, int* grid_out, int dry);
+
 struct FillLaunch {
   int G, R;
   // launches the variant for `flags`; smem/grid are computed inside. Returns the grid used.
   // dry != 0: nothing is launched, *grid_out = the warps of this variant resident on the whole GPU.
-  cudaError_t (*launch)(int flags, const FillParams& prm, uint32_t ntasks, int num_sms,
-                        cudaStream_t stream, int* grid_out, int dry);
+  FillLaunchFn launch;
+  // the F_NOTB variants (score-only batches), built for the shapes choose_shape picks; null for the others
+  FillLaunchFn launch_notb;
 };
 
 #define B2A_DECLARE_FILL(G, R)                                                                  \
   cudaError_t launch_fill_##G##_##R(int flags, const FillParams& prm, uint32_t ntasks,          \
                                     int num_sms, cudaStream_t stream, int* grid_out, int dry);
+#define B2A_DECLARE_FILL_NOTB(G, R)                                                             \
+  cudaError_t launch_fill_notb_##G##_##R(int flags, const FillParams& prm, uint32_t ntasks,     \
+                                         int num_sms, cudaStream_t stream, int* grid_out, int dry);
 
 B2A_DECLARE_FILL(1, 16)
 B2A_DECLARE_FILL(1, 8)
@@ -29,5 +36,10 @@ B2A_DECLARE_FILL(8, 16)
 B2A_DECLARE_FILL(8, 20)
 B2A_DECLARE_FILL(32, 8)
 B2A_DECLARE_FILL(32, 16)
+B2A_DECLARE_FILL_NOTB(1, 16)
+B2A_DECLARE_FILL_NOTB(8, 16)
+B2A_DECLARE_FILL_NOTB(8, 20)
+B2A_DECLARE_FILL_NOTB(32, 8)
+B2A_DECLARE_FILL_NOTB(32, 16)
 
 }  // namespace b2a

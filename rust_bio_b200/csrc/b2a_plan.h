@@ -35,10 +35,13 @@ struct Plan {
 
 inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 
-// `flags`: the fill's kernel flags (F_BND8 halves the boundary record)
+// `flags`: the fill's kernel flags (F_BND8 halves the boundary record; F_NOTB, a score-only batch, stores no
+// traceback, and its waves close on the rest of the per-wave scratch -- boundary rows, rows arena, row-m cells --
+// against the same budget)
 inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, uint64_t n_pairs, int G,
                        int R, uint64_t tb_budget, int flags = 0) {
   const uint64_t bnd_rec = (flags & F_BND8) ? 8 : 16;
+  const bool notb = (flags & F_NOTB) != 0;
   p.G = G;
   p.R = R;
   p.n_pairs = n_pairs;
@@ -98,8 +101,10 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     const uint64_t bnd = align_up((uint64_t)(k.maxn + 1) * 32 * bnd_rec, 256);
     const uint64_t rows = align_up((uint64_t)ROWS_ARRAYS * k.rows_pad * 32 * 4, 256);
     const uint64_t rowm = align_up((uint64_t)(k.maxn + 1) * 32 * 2, 256);
-    const uint64_t tb = align_up((uint64_t)G * k.nstrips * k.K * TBW * 512, 256);
-    if (b > w.block_lo && w.tb_bytes + tb > tb_budget) {  // close the wave
+    const uint64_t tb = notb ? 0 : align_up((uint64_t)G * k.nstrips * k.K * TBW * 512, 256);
+    const bool full = notb ? w.bnd_bytes + w.rows_bytes + w.rowm_bytes + bnd + rows + rowm > tb_budget
+                           : w.tb_bytes + tb > tb_budget;
+    if (b > w.block_lo && full) {  // close the wave
       w.block_hi = b;
       p.waves.push_back(w);
       w = Wave{b, b, 0, 0, 0, 0, 0};
@@ -118,7 +123,7 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     w.rows_bytes += rows;
     w.rowm_bytes += rowm;
     w.tb_bytes += tb;
-    p.total_tb += (uint64_t)G * k.nstrips * k.K * TBW * 512;
+    if (!notb) p.total_tb += (uint64_t)G * k.nstrips * k.K * TBW * 512;
   }
   if (nblocks) {
     w.block_hi = nblocks;

@@ -514,7 +514,12 @@ B2A_HD void walk_begin(const PairView& v, const EndState& es, uint8_t* ops_end, 
   w.ops_end = ops_end;
 }
 
-// returns true when the walk has ended (TB_START reached, or a panic path of the reference)
+// returns true when the walk has ended (TB_START reached, or a panic path of the reference).
+// SCORES (score-only batches, K1 ran with F_NOTB and left no interior traceback): xend / yend are assigned only by the
+// suffix-clip moves, whose S-codes sit on row m (x) and column n (y) only, and the walk never increases i or j -- so
+// the walk stops as soon as it stands on a cell with i < m and j < n, before it reads that cell's layer.  Until then
+// it reads row m, column n, the boundary row and the rows arena only.  It writes no ops (ops_end may be null).
+template <bool SCORES = false>
 B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_clips, WalkState& w, int32_t max_steps) {
   const DevScoring& sc = v.sc;
   const int32_t m = v.m, n = v.n;
@@ -529,6 +534,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
     if (i == 0) return row0_sbits(sc, j, n);
     if (i == m) return cell_s((uint32_t)v.rowm[j * 32 + v.pi]);
     if (j == 0) return col0_sbits(sc, i);
+    if (SCORES) return TB_START;  // an interior cell: the walk ends on it, its layer is never needed
     return v.nib_scode(v.nib(i, j), i, j);
   };
   int32_t i = w.i, j = w.j;
@@ -539,6 +545,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
   int32_t guard = w.guard;
   uint8_t* ops_end = w.ops_end;
   while (layer != TB_START && status == 0) {
+    if (SCORES && i < m && j < n) break;
     if (max_steps-- <= 0) break;
     if (--guard < 0) {
       status = 1;
@@ -546,7 +553,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
     }
     uint32_t next;
     if (layer == TB_INS) {
-      *(--ops_end) = 3;
+      if (!SCORES) *(--ops_end) =3;
       ++nops;
       uint32_t c;
       if (j == n) {
@@ -562,7 +569,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
       next = c;
       i -= 1;
     } else if (layer == TB_DEL) {
-      *(--ops_end) = 2;
+      if (!SCORES) *(--ops_end) =2;
       ++nops;
       uint32_t c;
       if (i == 0) {
@@ -578,14 +585,14 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
       next = c;
       j -= 1;
     } else if (layer == TB_MATCH || layer == TB_SUBST) {
-      *(--ops_end) = (layer == TB_MATCH) ? 0 : 1;
+      if (!SCORES) *(--ops_end) =(layer == TB_MATCH) ? 0 : 1;
       ++nops;
       next = get_s(i - 1, j - 1);
       i -= 1;
       j -= 1;
     } else if (layer == TB_XCLIP_PREFIX) {
       if (!filter_clips) {
-        *(--ops_end) = 4;
+        if (!SCORES) *(--ops_end) =4;
         ++nops;
         if (nclip < 4) clips[nclip] = (uint32_t)i;
         ++nclip;
@@ -599,7 +606,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
       else if (j == 0) lx = Lx0;
       else lx = (m >= 2) ? m - decode_boundary(v.load_bnd(j), v.packtrk != 0, v.bnd8 != 0, xs, m).Ti : 0;
       if (!filter_clips) {
-        *(--ops_end) = 4;
+        if (!SCORES) *(--ops_end) =4;
         ++nops;
         if (nclip < 4) clips[nclip] = (uint32_t)lx;
         ++nclip;
@@ -609,7 +616,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
       next = get_s(i, j);
     } else if (layer == TB_YCLIP_PREFIX) {
       if (!filter_clips) {
-        *(--ops_end) = 5;
+        if (!SCORES) *(--ops_end) =5;
         ++nops;
         if (nclip < 4) clips[nclip] = (uint32_t)j;
         ++nclip;
@@ -623,7 +630,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
       else if (i == 0 || n == 0) ly = n;
       else ly = n - v.row(ROWS_LY, i);
       if (!filter_clips) {
-        *(--ops_end) = 5;
+        if (!SCORES) *(--ops_end) =5;
         ++nops;
         if (nclip < 4) clips[nclip] = (uint32_t)ly;
         ++nclip;
@@ -654,7 +661,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
   for (int k = 0; k < 4; ++k) w.clips[k] = clips[k];
   w.guard = guard;
   w.ops_end = ops_end;
-  return layer == TB_START || status != 0;
+  return layer == TB_START || status != 0 || (SCORES && i < m && j < n);
 }
 
 B2A_HD void walk_finish(const EndState& es, const WalkState& w, WalkOut& out) {
@@ -671,12 +678,14 @@ B2A_HD void walk_finish(const EndState& es, const WalkState& w, WalkOut& out) {
 }
 
 // K2 for one pair by one lane: ops are written backwards into ops_end[-1], ops_end[-2], ...
+// (SCORES: score, xend, yend and status only, see walk_run; ops_end may be null)
+template <bool SCORES = false>
 B2A_HD void walk_pair(const PairView& v, const bool filter_clips, uint8_t* ops_end, WalkOut& out) {
   EndState es;
   finish_matrix_seq(v, es);
   WalkState w;
   walk_begin(v, es, ops_end, w);
-  walk_run(v, es, filter_clips, w, 0x7fffffff);
+  walk_run<SCORES>(v, es, filter_clips, w, 0x7fffffff);
   walk_finish(es, w, out);
 }
 
@@ -1084,8 +1093,8 @@ B2A_HD void prefetch_tb(const PairView& v, int32_t i, int32_t j) {
 #endif
 }
 
-// K2 for one pair by W cooperating lanes; `out` is complete on lane 0
-template <int W>
+// K2 for one pair by W cooperating lanes; `out` is complete on lane 0 (SCORES: as walk_pair, and no prefetches)
+template <int W, bool SCORES = false>
 B2A_HD void walk_pair_coop(const int lane, const PairView& v, const bool filter_clips, uint8_t* ops_end, WalkOut& out) {
   using C = Coop<W>;
   EndState es;
@@ -1095,10 +1104,12 @@ B2A_HD void walk_pair_coop(const int lane, const PairView& v, const bool filter_
   constexpr int32_t kBurst = 24;  // moves of lane 0 between two rounds of prefetches
   for (;;) {
     // every lane looks a different distance down the diagonal from where lane 0 stands
-    const int32_t ci = C::from(w.i, 0), cj = C::from(w.j, 0);
-    prefetch_tb(v, ci - 1 - lane, cj - 1 - lane);
+    if (!SCORES) {
+      const int32_t ci = C::from(w.i, 0), cj = C::from(w.j, 0);
+      prefetch_tb(v, ci - 1 - lane, cj - 1 - lane);
+    }
     int32_t done = 0;
-    if (lane == 0) done = walk_run(v, es, filter_clips, w, kBurst) ? 1 : 0;
+    if (lane == 0) done = walk_run<SCORES>(v, es, filter_clips, w, kBurst) ? 1 : 0;
     if (C::from(done, 0)) break;
   }
   walk_finish(es, w, out);
@@ -1106,7 +1117,36 @@ B2A_HD void walk_pair_coop(const int lane, const PairView& v, const bool filter_
 
 #if defined(__CUDACC__)
 
+// a pair's outputs (SCORES: score, xend, yend and status only; a score-only batch has no ops, starts or clips)
+template <bool SCORES>
+__device__ __forceinline__ void walk_store(const WalkParams& prm, const Block& blk, const uint32_t sp, const int pi,
+                                           const uint32_t cap, WalkOut& o) {
+  if (o.status) {  // the reference panics on this pair (mod.rs:905): no alignment is reported for it
+    o.score = MIN_SCORE;
+    o.n_ops = 0;
+    o.xstart = o.xend = o.ystart = o.yend = 0;
+    o.clip[0] = o.clip[1] = o.clip[2] = o.clip[3] = 0;
+  }
+  const uint32_t dst = prm.order[sp];
+  prm.score[dst] = o.score;
+  if (!SCORES) prm.xstart[dst] = o.xstart;
+  prm.xend[dst] = o.xend;
+  if (!SCORES) prm.ystart[dst] = o.ystart;
+  prm.yend[dst] = o.yend;
+  if (!SCORES) {
+    prm.n_ops[dst] = o.n_ops;
+    prm.ops_src[dst] = blk.ops_off + (uint64_t)(pi + 1) * cap - o.n_ops;
+  }
+  prm.status[dst] = o.status;
+  if (o.status) atomicOr(prm.err_flag, 1u);
+  if (!SCORES) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) prm.clip_len[4 * (size_t)dst + k] = o.clip[k];
+  }
+}
+
 // K2 for one pair (lane) of a block
+template <bool SCORES>
 __device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& blk, const int lane) {
   if ((uint32_t)lane >= blk.npairs) return;
   const uint32_t sp = blk.first + lane;
@@ -1137,30 +1177,14 @@ __device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& bl
   v.rowm = reinterpret_cast<uint16_t*>(prm.rowm + blk.rowm_off);
   v.tb = reinterpret_cast<const uint32_t*>(prm.tb + blk.tb_off);
   const uint32_t cap = blk.maxm + blk.maxn + 4;
-  uint8_t* ops_end = prm.ops_scratch + blk.ops_off + (size_t)(lane + 1) * cap;
+  uint8_t* ops_end = SCORES ? nullptr : prm.ops_scratch + blk.ops_off + (size_t)(lane + 1) * cap;
   WalkOut o;
-  walk_pair(v, prm.filter_clips != 0, ops_end, o);
-  if (o.status) {  // the reference panics on this pair (mod.rs:905): no alignment is reported for it
-    o.score = MIN_SCORE;
-    o.n_ops = 0;
-    o.xstart = o.xend = o.ystart = o.yend = 0;
-    o.clip[0] = o.clip[1] = o.clip[2] = o.clip[3] = 0;
-  }
-  const uint32_t dst = prm.order[sp];
-  prm.score[dst] = o.score;
-  prm.xstart[dst] = o.xstart;
-  prm.xend[dst] = o.xend;
-  prm.ystart[dst] = o.ystart;
-  prm.yend[dst] = o.yend;
-  prm.n_ops[dst] = o.n_ops;
-  prm.ops_src[dst] = blk.ops_off + (uint64_t)(lane + 1) * cap - o.n_ops;
-  prm.status[dst] = o.status;
-  if (o.status) atomicOr(prm.err_flag, 1u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) prm.clip_len[4 * (size_t)dst + k] = o.clip[k];
+  walk_pair<SCORES>(v, prm.filter_clips != 0, ops_end, o);
+  walk_store<SCORES>(prm, blk, sp, lane, cap, o);
 }
 
 // K2, one warp per pair
+template <bool SCORES>
 __device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& blk, const int pi, const int lane,
                                           uint8_t* seq_smem) {
   const uint32_t sp = blk.first + pi;
@@ -1201,31 +1225,17 @@ __device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& bl
     v.ys8 = reinterpret_cast<const uint8_t*>(ys);
   }
   const uint32_t cap = blk.maxm + blk.maxn + 4;
-  uint8_t* ops_end = prm.ops_scratch + blk.ops_off + (size_t)(pi + 1) * cap;
+  uint8_t* ops_end = SCORES ? nullptr : prm.ops_scratch + blk.ops_off + (size_t)(pi + 1) * cap;
   WalkOut o;
-  walk_pair_coop<32>(lane, v, prm.filter_clips != 0, ops_end, o);
+  walk_pair_coop<32, SCORES>(lane, v, prm.filter_clips != 0, ops_end, o);
   if (lane != 0) return;
-  if (o.status) {  // the reference panics on this pair (mod.rs:905): no alignment is reported for it
-    o.score = MIN_SCORE;
-    o.n_ops = 0;
-    o.xstart = o.xend = o.ystart = o.yend = 0;
-    o.clip[0] = o.clip[1] = o.clip[2] = o.clip[3] = 0;
-  }
-  const uint32_t dst = prm.order[sp];
-  prm.score[dst] = o.score;
-  prm.xstart[dst] = o.xstart;
-  prm.xend[dst] = o.xend;
-  prm.ystart[dst] = o.ystart;
-  prm.yend[dst] = o.yend;
-  prm.n_ops[dst] = o.n_ops;
-  prm.ops_src[dst] = blk.ops_off + (uint64_t)(pi + 1) * cap - o.n_ops;
-  prm.status[dst] = o.status;
-  if (o.status) atomicOr(prm.err_flag, 1u);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) prm.clip_len[4 * (size_t)dst + k] = o.clip[k];
+  walk_store<SCORES>(prm, blk, sp, pi, cap, o);
 }
 
 #if defined(B2A_DEFINE_WALK_KERNEL)  // one translation unit (b2a_engine.cu) owns the stand-alone kernel
+// SCORES: the score-only K2 of batches filled with F_NOTB (tb == null; xstart, ystart, n_ops, ops_src, clip_len and
+// ops_scratch are not written and may be null)
+template <bool SCORES>
 __global__ void __launch_bounds__(1024, 1) walk_warp_kernel(const WalkParams prm) {  // 64 registers; CTAs of 1..32 warps
   extern __shared__ __align__(16) uint8_t walk_smem[];  // seq_smem_per_warp bytes per warp, or none
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;  // one warp per (block, pair)
@@ -1235,15 +1245,16 @@ __global__ void __launch_bounds__(1024, 1) walk_warp_kernel(const WalkParams prm
   const Block blk = prm.blocks[b];
   if (pi >= blk.npairs) return;
   uint8_t* mine = prm.seq_smem_per_warp ? walk_smem + (size_t)(threadIdx.x >> 5) * prm.seq_smem_per_warp : nullptr;
-  walk_warp(prm, blk, (int)pi, lane, mine);
+  walk_warp<SCORES>(prm, blk, (int)pi, lane, mine);
 }
 
+template <bool SCORES>
 __global__ void __launch_bounds__(128, 8) walk_kernel(const WalkParams prm) {
   const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (gw >= prm.nblocks) return;
   const Block blk = prm.blocks[gw];
-  walk_lane(prm, blk, lane);
+  walk_lane<SCORES>(prm, blk, lane);
 }
 #endif
 

@@ -68,6 +68,23 @@ class Results:
         return {k: getattr(self, k) for k in ("score", "xstart", "xend", "ystart", "yend")}
 
 
+class ScoreResults:
+    """Host outputs of a score-only batch: score, xend, yend and the per-pair B2A_PAIR_* status (numpy arrays in the
+    caller's pair order); the other b2a_results fields stay NULL."""
+
+    def __init__(self, n_pairs: int):
+        self.n_pairs = n_pairs
+        self.score = np.zeros(max(1, n_pairs), dtype=np.int32)
+        self.xend = np.zeros(max(1, n_pairs), dtype=np.uint32)
+        self.yend = np.zeros(max(1, n_pairs), dtype=np.uint32)
+        self.status = np.zeros(max(1, n_pairs), dtype=np.uint32)
+        p = lambda a: a.ctypes.data_as(C.c_void_p)
+        self.c = CResults(p(self.score), None, p(self.xend), None, p(self.yend), None, None, 0, None, p(self.status))
+
+    def as_dict(self):
+        return {k: getattr(self, k)[:self.n_pairs] for k in ("score", "xend", "yend", "status")}
+
+
 class Engine:
     def __init__(self, device: int = 0):
         self._L = _lib.load()
@@ -140,6 +157,27 @@ class Engine:
         self._check(self._L.b2a_align_batch(self._h, int(mode), C.byref(cscoring), C.byref(cp),
                                             C.byref(results.c), C.byref(self.stats)))
         return results
+
+    def align_batch_scores(self, mode: int, cscoring: CScoring, batch: Batch) -> Dict[str, np.ndarray]:
+        """b2a_align_batch_scores: Alignment.score / xend / yend without the traceback -> {score, xend, yend, status}
+        (numpy, caller's pair order; a pair the reference panics on has status B2A_PAIR_PANIC)."""
+        res = ScoreResults(len(batch[2]))
+        cp = self._cpairs(batch)
+        self._check(self._L.b2a_align_batch_scores(self._h, int(mode), C.byref(cscoring), C.byref(cp),
+                                                   C.byref(res.c), C.byref(self.stats)))
+        return res.as_dict()
+
+    def stage_scores(self, mode: int, cscoring: CScoring, batch: Batch):
+        """b2a_batch_stage_scores: stage a score-only batch (then run(), fetch_scores())."""
+        self._keep = (batch, cscoring)
+        cp = self._cpairs(batch)
+        self._check(self._L.b2a_batch_stage_scores(self._h, int(mode), C.byref(cscoring), C.byref(cp)))
+
+    def fetch_scores(self) -> Dict[str, np.ndarray]:
+        """b2a_batch_fetch of a score-only batch -> {score, xend, yend, status}."""
+        res = ScoreResults(len(self._keep[0][2]))
+        self._check(self._L.b2a_batch_fetch(self._h, C.byref(res.c), C.byref(self.stats)))
+        return res.as_dict()
 
     def align_batch_banded(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch,
                            results: Optional[Results] = None) -> Results:

@@ -19,7 +19,7 @@ from ._lib import (CScoring, MIN_SCORE, MODE_CUSTOM, MODE_GLOBAL, MODE_LOCAL, MO
 from .alignment import Alignment, AlignmentMode, AlignmentOperation
 from .engine import Engine, Results, default_engine, pack_pairs
 
-__all__ = ["MIN_SCORE", "MatchParams", "Scoring", "Aligner", "MatchFunc"]
+__all__ = ["MIN_SCORE", "MatchParams", "Scoring", "Aligner", "MatchFunc", "AlignmentScore"]
 
 MatchFunc = Union["MatchParams", Callable[[int, int], int]]
 DEFAULT_ALIGNER_CAPACITY = 200  # mod.rs:483
@@ -144,6 +144,14 @@ def _symbols_present(batch) -> np.ndarray:
     return np.nonzero(np.bincount(blob[inside], minlength=256))[0].astype(np.uint8)
 
 
+@dataclass(frozen=True)
+class AlignmentScore:
+    """What a score-only call returns per pair: Alignment.score, xend and yend (no start coordinates, no ops)."""
+    score: int
+    xend: int
+    yend: int
+
+
 _PAIR_STATUS_TEXT = {1: "the reference panics (or never returns) on this pair: mod.rs:905 / banded.rs:777-831",
                      2: "banded: more k-mer matches than the engine's per-pair limit",
                      4: "banded: the reference panics on these caller-supplied matches/path"}
@@ -237,6 +245,37 @@ class Aligner:
         self.engine.align_batch_packed(mode, cs, packed, results=res)
         fake = [(b"\0" * a, b"\0" * b) for a, b in lens]  # _alignments only needs the lengths
         return _alignments(res, fake, mode, on_panic)
+
+    def _scores_batch(self, mode: int, pairs: Sequence[Tuple[bytes, bytes]], on_panic: str = "raise"):
+        """Alignment.score / xend / yend of each pair without the traceback (b2a_align_batch_scores): what the full
+        call returns in those fields.  on_panic as in _batch; a panic only the traceback's interior would meet
+        cannot be seen here, and such a pair reports its score (include/b200align.h)."""
+        from ._lib import B2AError
+        batch = pack_pairs(pairs)
+        cs, keep = self.scoring.to_c(batch)
+        res = self.engine.align_batch_scores(mode, cs, batch)
+        out = []
+        for i in range(len(pairs)):
+            st = int(res["status"][i])
+            if st:
+                if on_panic == "raise":
+                    raise B2AError(-4, f"pair {i}: " + _PAIR_STATUS_TEXT.get(st, str(st)))
+                out.append(None)
+                continue
+            out.append(AlignmentScore(int(res["score"][i]), int(res["xend"][i]), int(res["yend"][i])))
+        return out
+
+    def custom_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional["AlignmentScore"]]:
+        return self._scores_batch(MODE_CUSTOM, pairs, on_panic)
+
+    def global_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional["AlignmentScore"]]:
+        return self._scores_batch(MODE_GLOBAL, pairs, on_panic)
+
+    def semiglobal_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional["AlignmentScore"]]:
+        return self._scores_batch(MODE_SEMIGLOBAL, pairs, on_panic)
+
+    def local_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional["AlignmentScore"]]:
+        return self._scores_batch(MODE_LOCAL, pairs, on_panic)
 
     def custom_batch(self, pairs, on_panic: str = "raise"):
         return self._batch(MODE_CUSTOM, pairs, on_panic)

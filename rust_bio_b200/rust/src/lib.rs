@@ -91,6 +91,14 @@ pub mod alignment {
                 results: *mut b2a_results,
                 stats: *mut c_void,
             ) -> i32;
+            fn b2a_align_batch_scores(
+                e: *mut c_void,
+                mode: i32,
+                scoring: *const b2a_scoring,
+                pairs: *const b2a_pairs,
+                results: *mut b2a_results,
+                stats: *mut c_void,
+            ) -> i32;
             fn b2a_align_batch_banded(
                 e: *mut c_void,
                 mode: i32,
@@ -252,6 +260,40 @@ pub mod alignment {
         }
         unsafe impl<F: MatchFunc + Send> Send for Aligner<F> {}
 
+        /// What a `*_scores_batch` call returns per pair: `Alignment::{score, xend, yend}` (no start coordinates, no
+        /// operations: those come out of the traceback, which a score-only batch does not keep).
+        #[derive(Clone, Copy, Debug, PartialEq, Eq)]
+        pub struct AlignmentScore {
+            pub score: i32,
+            pub xend: usize,
+            pub yend: usize,
+        }
+
+        /// A batch in the C ABI's input layout (owned; `c_pairs` borrows it)
+        struct PackedBatch {
+            blob: Vec<u8>,
+            x_off: Vec<u64>,
+            y_off: Vec<u64>,
+            x_len: Vec<u32>,
+            y_len: Vec<u32>,
+            table: Vec<i32>,
+            alphabet: Vec<u8>,
+        }
+
+        impl PackedBatch {
+            fn c_pairs(&self) -> b2a_pairs {
+                b2a_pairs {
+                    seq_blob: self.blob.as_ptr(),
+                    x_off: self.x_off.as_ptr(),
+                    x_len: self.x_len.as_ptr(),
+                    y_off: self.y_off.as_ptr(),
+                    y_len: self.y_len.as_ptr(),
+                    blob_bytes: self.blob.len() as u64,
+                    n_pairs: self.x_len.len() as u64,
+                }
+            }
+        }
+
         impl<F: MatchFunc> Drop for Aligner<F> {
             fn drop(&mut self) {
                 unsafe {
@@ -304,10 +346,10 @@ pub mod alignment {
                 self
             }
 
-            /// Aligner::custom / global / semiglobal / local over a batch (mode = B2A_MODE_*).
-            pub(crate) fn batch(&mut self, mode: i32, banded: Option<BandedCall>, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> {
+            /// The batch in the C ABI's input layout: 16-byte aligned slots (x then y per pair), and the MatchFunc
+            /// tabulated over the symbols present (mod.rs:221-228 allows any closure).
+            fn pack(&self, pairs: &[(&[u8], &[u8])]) -> PackedBatch {
                 let n = pairs.len();
-                // 16-byte aligned slots, x then y per pair
                 let mut x_off = Vec::with_capacity(n);
                 let mut y_off = Vec::with_capacity(n);
                 let mut x_len = Vec::with_capacity(n);
@@ -328,7 +370,6 @@ pub mod alignment {
                     x_len.push(x.len() as u32);
                     y_len.push(y.len() as u32);
                 }
-                // tabulate the MatchFunc over the symbols present (mod.rs:221-228 allows any closure)
                 let alphabet: Vec<u8> = (0..=255u8).filter(|b| present[*b as usize]).collect();
                 let mut table = vec![0i32; 256 * 256];
                 for &a in &alphabet {
@@ -336,8 +377,12 @@ pub mod alignment {
                         table[a as usize * 256 + b as usize] = self.scoring.match_fn.score(a, b);
                     }
                 }
+                PackedBatch { blob, x_off, y_off, x_len, y_len, table, alphabet }
+            }
+
+            fn c_scoring(&self, pb: &PackedBatch) -> b2a_scoring {
                 let (ms, mm) = self.scoring.match_scores.unwrap_or((0, 0));
-                let cs = b2a_scoring {
+                b2a_scoring {
                     gap_open: self.scoring.gap_open,
                     gap_extend: self.scoring.gap_extend,
                     xclip_prefix: self.scoring.xclip_prefix,
@@ -347,19 +392,17 @@ pub mod alignment {
                     match_score: ms,
                     mismatch_score: mm,
                     has_match_scores: self.scoring.match_scores.is_some() as i32,
-                    table: table.as_ptr(),
-                    alphabet: alphabet.as_ptr(),
-                    alphabet_len: alphabet.len() as u32,
-                };
-                let cp = b2a_pairs {
-                    seq_blob: blob.as_ptr(),
-                    x_off: x_off.as_ptr(),
-                    x_len: x_len.as_ptr(),
-                    y_off: y_off.as_ptr(),
-                    y_len: y_len.as_ptr(),
-                    blob_bytes: blob.len() as u64,
-                    n_pairs: n as u64,
-                };
+                    table: pb.table.as_ptr(),
+                    alphabet: pb.alphabet.as_ptr(),
+                    alphabet_len: pb.alphabet.len() as u32,
+                }
+            }
+
+            /// Aligner::custom / global / semiglobal / local over a batch (mode = B2A_MODE_*).
+            pub(crate) fn batch(&mut self, mode: i32, banded: Option<BandedCall>, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> {
+                let n = pairs.len();
+                let pb = self.pack(pairs);
+                let (cs, cp) = (self.c_scoring(&pb), pb.c_pairs());
                 let cap: u64 = pairs.iter().map(|(x, y)| (x.len() + y.len() + 4) as u64).sum();
                 let mut score = vec![0i32; n];
                 let (mut xs, mut xe, mut ys, mut ye) = (vec![0u32; n], vec![0u32; n], vec![0u32; n], vec![0u32; n]);
@@ -481,6 +524,39 @@ pub mod alignment {
             pub fn global_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { self.batch(1, None, pairs) }
             pub fn semiglobal_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { self.batch(2, None, pairs) }
             pub fn local_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { self.batch(3, None, pairs) }
+
+            /// Alignment::{score, xend, yend} of each pair without the traceback (b2a_align_batch_scores), on this
+            /// aligner's device.  Panics where the full call would (a pair the reference panics on).
+            pub(crate) fn scores_batch(&mut self, mode: i32, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> {
+                let n = pairs.len();
+                let pb = self.pack(pairs);
+                let (cs, cp) = (self.c_scoring(&pb), pb.c_pairs());
+                let mut score = vec![0i32; n.max(1)];
+                let (mut xe, mut ye) = (vec![0u32; n.max(1)], vec![0u32; n.max(1)]);
+                let mut res = b2a_results {
+                    score: score.as_mut_ptr(),
+                    xstart: std::ptr::null_mut(),
+                    xend: xe.as_mut_ptr(),
+                    ystart: std::ptr::null_mut(),
+                    yend: ye.as_mut_ptr(),
+                    ops_off: std::ptr::null_mut(),
+                    ops: std::ptr::null_mut(),
+                    ops_capacity: 0,
+                    clip_len: std::ptr::null_mut(),
+                    status: std::ptr::null_mut(),
+                };
+                let rc = unsafe { b2a_align_batch_scores(self.engine, mode, &cs, &cp, &mut res, std::ptr::null_mut()) };
+                if rc != 0 {
+                    let msg = unsafe { CStr::from_ptr(b2a_last_error(self.engine)) }.to_string_lossy().into_owned();
+                    panic!("{}", msg);
+                }
+                (0..n).map(|p| AlignmentScore { score: score[p], xend: xe[p] as usize, yend: ye[p] as usize }).collect()
+            }
+
+            pub fn custom_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(0, pairs) }
+            pub fn global_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(1, pairs) }
+            pub fn semiglobal_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(2, pairs) }
+            pub fn local_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(3, pairs) }
 
             /// mod.rs:591
             pub fn custom(&mut self, x: &[u8], y: &[u8]) -> Alignment { self.batch(0, None, &[(x, y)]).remove(0) }
