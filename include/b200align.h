@@ -202,7 +202,8 @@ int32_t b2a_align_batch(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
  * A forced fill shape (b2a_engine_set_tuning) other than 1x16, 8x16, 8x20, 32x8 or 32x16 is B2A_E_UNSUPPORTED.
  * status: a pair whose walk would panic or never end while still on row m / column n is B2A_PAIR_PANIC, as with
  * b2a_align_batch.  A panic only the interior walk would meet (mod.rs:905) cannot be seen without the traceback:
- * such a pair reports its score. */
+ * such a pair reports its score.
+ * The banded aligner's score-only form, under the same rule, is b2a_align_batch_banded_scores (below). */
 int32_t b2a_batch_stage_scores(b2a_engine* e, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs);
 int32_t b2a_align_batch_scores(b2a_engine* e, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
                                b2a_results* results, b2a_stats* stats);
@@ -258,6 +259,20 @@ typedef struct b2a_band_hints {
 int32_t b2a_align_batch_banded_hinted(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
                                       uint32_t k, uint32_t w, const b2a_pairs* pairs,
                                       const b2a_band_hints* hints, b2a_results* results, b2a_stats* stats);
+
+/* banded::Aligner reduced to Alignment.score / xend / yend, as b2a_align_batch_scores is for Aligner: hints == NULL is
+ * b2a_align_batch_banded, non-NULL hints are b2a_align_batch_banded_hinted (same validation and refusals).  For each
+ * pair, score, xend and yend are what the full call returns.  The band (K4), the path every pair takes and the
+ * per-pair statuses B2A_PAIR_CAPACITY / B2A_PAIR_INVALID_HINT are the full call's; a band above MAX_CELLS returns
+ * MIN_SCORE, 0, 0 as there.  No interior traceback cell (1 <= i < m, 1 <= j < n) is stored, and the walk stops on the
+ * first cell with i < m and j < n: xend and yend are set only by the suffix-clip moves, whose codes sit on row m and
+ * column n, and the walk never increases i or j.  results: score, xend, yend and status; xstart, ystart, ops, ops_off
+ * and clip_len must be NULL (else B2A_E_INVALID).  b2a_banded_band_ranges and b2a_banded_strip_pairs work after it
+ * as after a full call.  status: a panic met on row m / column n is B2A_PAIR_PANIC; one only the interior walk would
+ * meet (banded.rs:777-831) cannot be seen without the traceback, and such a pair reports its score. */
+int32_t b2a_align_batch_banded_scores(b2a_engine* e, int32_t mode, const b2a_scoring* scoring, uint32_t k, uint32_t w,
+                                      const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
+                                      b2a_stats* stats);
 
 /* Band::ranges of one pair of the last banded call (what banded::Aligner::visualize draws, banded.rs:1007-1030):
  * y_len + 1 half-open row ranges as (start, end) u32 pairs; an empty column is (x_len + 1, 0) (banded.rs:1065).

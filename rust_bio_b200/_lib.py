@@ -25,7 +25,7 @@ ABI_SYMBOLS = [
     "b2a_engine_set_stream", "b2a_engine_set_traceback_budget", "b2a_engine_set_tuning",
     "b2a_engine_set_pipeline", "b2a_engine_set_walk", "b2a_engine_last_alphabet",
     "b2a_align_batch", "b2a_align_batch_banded", "b2a_align_batch_banded_hinted", "b2a_banded_band_ranges", "b2a_banded_strip_pairs", "b2a_batch_stage", "b2a_batch_run",
-    "b2a_batch_stage_scores", "b2a_align_batch_scores",
+    "b2a_batch_stage_scores", "b2a_align_batch_scores", "b2a_align_batch_banded_scores",
     "b2a_batch_fetch", "b2a_batch_records", "b2a_batch_records_into", "b2a_record_stride",
     "b2a_records_decode", "b2a_batch_compact_bytes", "b2a_batch_compact_into", "b2a_compact_decode",
     "b2a_batch_compact_fixed", "b2a_gathered_fetch", "b2a_align_batch_packed", "b2a_align_batch_banded_packed",
@@ -115,6 +115,9 @@ def load():
                                          C.c_uint32, C.POINTER(CPairs), C.POINTER(CResults),
                                          C.POINTER(CStats)]
     L.b2a_align_batch_banded_hinted.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.c_uint32,
+                                                C.c_uint32, C.POINTER(CPairs), C.POINTER(CBandHints),
+                                                C.POINTER(CResults), C.POINTER(CStats)]
+    L.b2a_align_batch_banded_scores.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.c_uint32,
                                                 C.c_uint32, C.POINTER(CPairs), C.POINTER(CBandHints),
                                                 C.POINTER(CResults), C.POINTER(CStats)]
     L.b2a_banded_band_ranges.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]

@@ -19,7 +19,8 @@ from typing import List, Optional, Sequence, Tuple
 from ._lib import MIN_SCORE, MODE_CUSTOM, MODE_GLOBAL, MODE_LOCAL, MODE_SEMIGLOBAL
 from .alignment import Alignment, AlignmentMode, AlignmentOperation
 from .engine import Engine, Results, default_engine, pack_pairs
-from .pairwise import DEFAULT_ALIGNER_CAPACITY, MatchFunc, Scoring, _alignments, _check_scoring
+from .pairwise import (DEFAULT_ALIGNER_CAPACITY, AlignmentScore, MatchFunc, Scoring, _alignment_scores, _alignments,
+                       _check_scoring)
 
 MAX_CELLS = 5_000_000          # banded.rs:104
 DEFAULT_MATCH_SCORE = 2        # banded.rs:105
@@ -74,6 +75,28 @@ class Aligner:
         self.engine.align_batch_banded_hinted(MODE_CUSTOM, cs, self.k, self.w, batch, matches, paths,
                                               allowed_mismatches, use_lcskpp_union, results=res)
         return _alignments(res, pairs, MODE_CUSTOM, on_panic, banded=True, result_mode=AlignmentMode.Custom)
+
+    def _scores_batch(self, mode: int, pairs, on_panic: str = "raise") -> List[Optional[AlignmentScore]]:
+        """Alignment.score / xend / yend of each pair without the traceback (b2a_align_batch_banded_scores): what the
+        `*_batch` form returns in those fields; a band above MAX_CELLS gives (MIN_SCORE, 0, 0).  on_panic as in
+        _batch; a panic only the traceback's interior would meet cannot be seen here, and such a pair reports its
+        score (include/b200align.h)."""
+        batch = pack_pairs(pairs)
+        cs, keep = self.scoring.to_c(batch)
+        res = self.engine.align_batch_banded_scores(mode, cs, self.k, self.w, batch)
+        return _alignment_scores(res, len(pairs), on_panic)
+
+    def custom_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional[AlignmentScore]]:
+        return self._scores_batch(MODE_CUSTOM, pairs, on_panic)
+
+    def global_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional[AlignmentScore]]:
+        return self._scores_batch(MODE_GLOBAL, pairs, on_panic)
+
+    def semiglobal_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional[AlignmentScore]]:
+        return self._scores_batch(MODE_SEMIGLOBAL, pairs, on_panic)
+
+    def local_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional[AlignmentScore]]:
+        return self._scores_batch(MODE_LOCAL, pairs, on_panic)
 
     def visualize(self, alignment: Alignment, file=None) -> str:
         """banded.rs:1007-1030: the band of the LAST single-pair alignment ('x'), the alignment's path ('\\'), one

@@ -73,6 +73,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
     esrc = os.path.join(CSRC, "b2a_engine.cu")
     if force or _stale(eo, hdrs + [esrc]):
         jobs.append([NVCC, *FLAGS, "-c", esrc, "-o", eo])
+    so = os.path.join(OBJ, "banded_strip_notb.o")  # the strip fill's score-only twins, beside engine.o
+    objs.append(so)
+    ssrc = os.path.join(CSRC, "b2a_banded_strip_notb.cu")
+    if force or _stale(so, hdrs + [ssrc]):
+        jobs.append([NVCC, *FLAGS, "-c", ssrc, "-o", so])
     mo = os.path.join(OBJ, "multi.o")
     objs.append(mo)
     msrc = os.path.join(CSRC, "b2a_multi.cu")

@@ -1007,9 +1007,10 @@ B2A_HD K3Layout k3_layout(uint64_t m, uint64_t n, uint64_t ncells) {
   L.total = (b + 255) & ~255ull;
   return L;
 }
-B2A_HD uint64_t k3_slab_bytes(uint64_t m, uint64_t n, uint64_t cells) {
+// score_only: the slab of a score-only call has no interior cells (the region `cells` is empty)
+B2A_HD uint64_t k3_slab_bytes(uint64_t m, uint64_t n, uint64_t cells, bool score_only = false) {
   // a refused band (> MAX_CELLS) needs no state at all
-  return cells > BANDED_MAX_CELLS ? 256 : k3_layout(m, n, cells).total;
+  return cells > BANDED_MAX_CELLS ? 256 : k3_layout(m, n, score_only ? 0 : cells).total;
 }
 
 struct BandedOut {
@@ -1124,7 +1125,8 @@ B2A_HD int32_t count_trailing_ones(uint32_t v) {  // number of consecutive set b
 #endif
 }
 
-template <int W, int R, class ScoreFn>
+// SCORES: no interior cell is stored (`cells` may be null); column n's cells, the border rows, Sn/Ly and Lx are as above
+template <int W, int R, class ScoreFn, bool SCORES = false>
 B2A_HD void banded_columns_fast(const int lane, const uint8_t* x, const int32_t m, const uint8_t* y, const int32_t n,
                                 const DevScoring& sc, ScoreFn score, const uint32_t* rng, const uint32_t* colstart,
                                 const int32_t* S0arr /* column 0's S */, int32_t* Sfin, int32_t* Ifin, int32_t* Sn,
@@ -1350,7 +1352,7 @@ B2A_HD void banded_columns_fast(const int lane, const uint8_t* x, const int32_t 
       const uint32_t up_sb = (uint32_t)C::from((int32_t)sb[R - 1], prev_lane);
       const int32_t up_sncur = last ? C::from(sncur[R - 1], prev_lane) : MIN_SCORE;
       uint16_t* const wbase = last ? coln : cells;
-      const uint32_t woff = last ? 0u : colstart[j] - (uint32_t)s;  // cell (i, j) = wbase[woff + i]
+      const uint32_t woff = (last || SCORES) ? 0u : colstart[j] - (uint32_t)s;  // cell (i, j) = wbase[woff + i]
       int32_t lane_trk_val = MIN_SCORE, lane_trk_i = 0;
 #pragma unroll
       for (int r = 0; r < R; ++r) {
@@ -1387,7 +1389,7 @@ B2A_HD void banded_columns_fast(const int lane, const uint8_t* x, const int32_t 
           }
           if (last && pSn + go > bl) ib = TB_YCLIP_SUFFIX;
         }
-        wbase[woff + (uint32_t)i] = (uint16_t)(ib | (db[r] << 4) | (sb[r] << 8));
+        if (!SCORES || last) wbase[woff + (uint32_t)i] = (uint16_t)(ib | (db[r] << 4) | (sb[r] << 8));
         if (last) {  // the end-of-matrix passes read column n's S and I from the slab
           Sfin[i] = best[r];
           Ifin[i] = best_i[r];
@@ -1590,7 +1592,13 @@ B2A_HD void banded_columns_fast(const int lane, const uint8_t* x, const int32_t 
 // PHASE: 0 = the whole alignment; 1 = everything up to the final score (left in S[n % 2][m]); 2 = the walk only, on
 // the state phase 1 left in the slab (the strip path walks one pair per LANE in a kernel of its own: the walk is
 // sequential per pair, and a warp whose other 31 lanes wait for lane 0 issues 32 times the instructions).
-template <int W, class ScoreFn, int FASTR = 0, int PHASE = 0>
+// SCORES (score-only calls): score, xend, yend and status only.  No interior cell (1 <= i <= m-1, 1 <= j <= n-1) is
+// stored or read -- the slab has no `cells` region, the strip area no traceback -- and a read of one returns START
+// without touching memory; row 0, row m, column 0, column n, Sn/Ly/Lx and the end-of-matrix passes are as above.
+// xend / yend are set only by the suffix-clip moves, whose codes sit on row m and column n, and the walk never
+// increases i or j: it stops on the first cell with i < m and j < n, before reading it (DESIGN.md §2).  It writes no
+// ops (ops_end may be null), no starts and no clip lengths.
+template <int W, class ScoreFn, int FASTR = 0, int PHASE = 0, bool SCORES = false>
 B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8_t* y, uint64_t n,
                              const DevScoring& sc, ScoreFn score, const uint32_t* rng, uint64_t num_cells,
                              uint8_t* slab, bool filter_clips, uint8_t* ops_end, BandedOut& out,
@@ -1607,7 +1615,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
   }
   out.xlen = (uint32_t)m;
   out.ylen = (uint32_t)n;
-  const K3Layout L = k3_layout(m, n, num_cells);
+  const K3Layout L = k3_layout(m, n, SCORES ? 0 : num_cells);
   uint32_t* colstart = reinterpret_cast<uint32_t*>(slab + L.colstart);
   int32_t* S0 = reinterpret_cast<int32_t*>(slab + L.S);
   int32_t* Sarr[2] = {S0, S0 + (m + 1)};
@@ -1628,7 +1636,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
   }
   if constexpr (PHASE != 2) {
   // init (banded.rs:423-438): only the cells that can ever be non-START are stored
-  if (!STRIP) {
+  if (!STRIP && !SCORES) {
     uint32_t acc = 0;  // exclusive prefix sum of the column heights
     for (uint64_t b = 0; b <= n; b += W) {
       const uint64_t j = b + (uint64_t)lane;
@@ -1686,7 +1694,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
     if (i == m) return &rowm[j];
     if (j == 0) return &col0[i];
     if (j == n) return &coln[i];
-    if (STRIP) return nullptr;  // interior cells live in the 4-bit traceback, nothing writes them here
+    if (STRIP || SCORES) return nullptr;  // interior cells live in the 4-bit traceback (or nowhere), nothing writes them here
     const uint64_t s = rng[2 * j], e = rng[2 * j + 1];
     if (i >= s && i < e) return &cells[colstart[j] + (i - s)];
     return nullptr;
@@ -1728,6 +1736,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
     }
   };
   auto sbits_at = [&](uint64_t i, uint64_t j) -> uint32_t {
+    if (SCORES && i >= 1 && i < m && j >= 1 && j < n) return 0u;
     if (STRIP && i >= 1 && i < m && j >= 1 && j < n) {
       const uint32_t nb = ks_nib(i, j);
       return nb == 16u ? 0u : ks_sbits(i, j, nb);
@@ -1738,6 +1747,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
   // one field of a cell (0: i-bits, 1: d-bits, 2: s-bits); in the 4-bit traceback "came from S of the neighbour"
   // resolves to that neighbour's s-bits (untouched cells read as START)
   auto rd_part = [&](uint64_t i, uint64_t j, int part) -> uint32_t {
+    if (SCORES && i >= 1 && i < m && j >= 1 && j < n) return 0u;
     if (STRIP && i >= 1 && i < m && j >= 1 && j < n) {
       const uint32_t nb = ks_nib(i, j);
       if (nb == 16u) return 0u;
@@ -1821,8 +1831,8 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
   C::sync();
   uint64_t lit_from = 1;  // first column of the literal loop below
   if constexpr (FASTR > 0) {
-    banded_columns_fast<W, FASTR>(lane, x, (int32_t)m, y, (int32_t)n, sc, score, rng, colstart, Sarr[0], Sarr[n % 2],
-                                  Iarr[n % 2], Sn, Ly, Lx, row0, rowm, col0, coln, cells);
+    banded_columns_fast<W, FASTR, ScoreFn, SCORES>(lane, x, (int32_t)m, y, (int32_t)n, sc, score, rng, colstart, Sarr[0],
+                                                   Sarr[n % 2], Iarr[n % 2], Sn, Ly, Lx, row0, rowm, col0, coln, cells);
   } else if constexpr (FASTR < 0) {
     // ---------------------------------------------------------------------------------------------------------
     // Finish pass of the strip-wavefront fill: what the column loop (banded.rs:511-681) does outside the interior
@@ -2094,9 +2104,9 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
       const uint64_t jj = j - 1;
       const uint32_t ps = jj == 0 ? 0u : rng[2 * jj], pe = jj == 0 ? 0xFFFFFFFFu : rng[2 * jj + 1];
       const uint16_t* const pbase = jj == 0 ? col0 : cells;
-      const uint32_t poff = (jj == 0 || STRIP) ? 0u : colstart[jj] - ps;  // cell (i, j-1) = pbase[poff + i] for ps <= i < pe
+      const uint32_t poff = (jj == 0 || STRIP || SCORES) ? 0u : colstart[jj] - ps;  // cell (i, j-1) = pbase[poff + i] for ps <= i < pe
       uint16_t* const wbase = last ? coln : cells;
-      const uint32_t woff = last ? 0u : colstart[j] - (uint32_t)i_start;  // cell (i, j) = wbase[woff + i]
+      const uint32_t woff = (last || SCORES) ? 0u : colstart[j] - (uint32_t)i_start;  // cell (i, j) = wbase[woff + i]
       const uint32_t lo32 = (uint32_t)lo, hm32 = (uint32_t)hi_main;
       const int32_t ly_now = (int32_t)(n - j);
       for (uint32_t base = lo32; base < hm32; base += W) {
@@ -2116,7 +2126,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
           db = TB_DEL;
         } else {
           best_d = s_open;
-          if (STRIP && jj != 0) {  // (column n-1's interior cells live in the strip fill's 4-bit traceback)
+          if ((STRIP || SCORES) && jj != 0) {  // (column n-1's interior cells live in the strip fill's 4-bit traceback)
             db = sbits_at(ic, jj);
           } else {
             const uint32_t pc = (ic >= ps && ic < pe) ? (uint32_t)pbase[poff + ic] : 0u;
@@ -2198,7 +2208,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
           S[i] = best;
           I[i] = best_i;
           D[i] = best_d;
-          wbase[woff + i] = (uint16_t)(ib | (db << 4) | (sb << 8));
+          if (!SCORES || last) wbase[woff + i] = (uint16_t)(ib | (db << 4) | (sb << 8));
           // column tracker, this lane's share: its rows come in ascending order, so a strict > keeps the first
           if (best + xs > lane_trk_val) {
             lane_trk_val = best + xs;
@@ -2450,12 +2460,12 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
   uint32_t nops = 0, nclip = 0, clips[4] = {0, 0, 0, 0};
   const uint64_t ops_cap = m + n + 4;
   bool overflow = false;
-  auto push = [&](uint32_t code) {
+  auto push = [&](uint32_t code) {  // (SCORES: counted, not stored -- an overflow is still the reference's panic)
     if (nops >= ops_cap) {
       overflow = true;
       return;
     }
-    *(--ops_end) = (uint8_t)code;
+    if (!SCORES) *(--ops_end) = (uint8_t)code;
     ++nops;
   };
   auto push_clip = [&](uint32_t code, uint32_t len) {
@@ -2490,12 +2500,17 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
     if (!((uint32_t)ii >= bs && (uint32_t)ii < be)) return 16u;
     return (word >> (4u * (7u - (t & 7u)))) & 15u;
   };
+  bool interior = false;  // SCORES: the walk stopped on a cell with i < m and j < n
   while (layer != TB_START) {
+    if (SCORES && i < m && j < n) {
+      interior = true;
+      break;
+    }
     if (guard-- == 0 || overflow) {
       out.status = 1;
       break;
     }
-    if (STRIP && i >= 1 && i < m && j >= 1 && j < n &&
+    if (!SCORES && STRIP && i >= 1 && i < m && j >= 1 && j < n &&
         (layer == TB_INS || layer == TB_DEL || layer == TB_MATCH || layer == TB_SUBST)) {
       int32_t fi = (int32_t)i, fj = (int32_t)j;
       uint32_t nbc = nib32(fi, fj);
@@ -2610,7 +2625,7 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
     }
     layer = next;
   }
-  if (out.status == 0) {
+  if (out.status == 0 && !interior) {
     if (i != 0) {  // banded.rs:834-844
       const int32_t i_score = go + ge * ((int32_t)i - 1);
       if (i_score > xp) {
@@ -2634,16 +2649,17 @@ B2A_HD void banded_compute_d(int lane, const uint8_t* x, uint64_t m, const uint8
   }
   if (overflow) out.status = 1;
   if (nclip > 4) out.status = 1;
-  out.xstart = xstart;
   out.xend = xend;
-  out.ystart = ystart;
   out.yend = yend;
+  out.xstart = SCORES ? 0u : xstart;
+  out.ystart = SCORES ? 0u : ystart;
+  if (SCORES) return;  // (ops and clip lengths stay 0)
   out.n_ops = nops;
   const uint32_t nc = nclip > 4 ? 4 : nclip;
   for (uint32_t q = 0; q < 4; ++q) out.clip[q] = q < nc ? clips[nc - 1 - q] : 0u;
 }
 
-#if defined(__CUDACC__)
+#if defined(__CUDACC__) && !defined(B2A_BANDED_NO_KERNELS)  // (b2a_banded_strip_notb.cu: the device functions only)
 
 // K4: one warp per pair
 __global__ void __launch_bounds__(128) band_kernel(const BandedParams prm, uint32_t n_wave) {
@@ -2693,7 +2709,8 @@ __global__ void __launch_bounds__(128) band_kernel(const BandedParams prm, uint3
 #endif
 // K3: one warp per pair.  FASTR == 0: the literal column loop, for every pair K4 did not mark; FASTR > 0: the
 // register-resident loop, for the marked ones (each kernel skips the other's pairs).
-template <int FASTR, int PHASE = 0, int W = 32>
+// SCORES: a score-only call (banded_compute_d): score, xend, yend and status only; prm.ops_scratch may be null.
+template <int FASTR, int PHASE = 0, int W = 32, bool SCORES = false>
 __device__ __forceinline__ void banded_fill_body(const BandedParams& prm, uint32_t n_wave) {
   // W = 32: one warp per pair; W = 1 (the strip path's walk): one thread per pair
   const uint32_t t = W == 32 ? (blockIdx.x * blockDim.x + threadIdx.x) >> 5 : blockIdx.x * blockDim.x + threadIdx.x;
@@ -2735,10 +2752,10 @@ __device__ __forceinline__ void banded_fill_body(const BandedParams& prm, uint32
       }
       return a == b ? sc.match_score : sc.mismatch_score;
     };
-    banded_compute_d<W, decltype(score), FASTR, PHASE>(lane, prm.blob + prm.x_off[p], m, prm.blob + prm.y_off[p], n,
+    banded_compute_d<W, decltype(score), FASTR, PHASE, SCORES>(lane, prm.blob + prm.x_off[p], m, prm.blob + prm.y_off[p], n,
                                                        prm.sc, score, prm.ranges + prm.ranges_off[t] / 4, prm.num_cells[p],
                                                        prm.fill + prm.fill_off[t], prm.filter_clips != 0,
-                                                       prm.ops_scratch + prm.ops_off[p], o,
+                                                       SCORES ? nullptr : prm.ops_scratch + prm.ops_off[p], o,
                                                        FASTR < 0 ? prm.strip + prm.strip_off[t] : nullptr,
                                                        FASTR < 0 ? prm.band_cols + 3 * p : nullptr, &redo);
   }
@@ -2755,15 +2772,18 @@ __device__ __forceinline__ void banded_fill_body(const BandedParams& prm, uint32
     o.clip[0] = o.clip[1] = o.clip[2] = o.clip[3] = 0;
   }
   prm.score[p] = o.score;
-  prm.xstart[p] = o.xstart;
+  if (!SCORES) prm.xstart[p] = o.xstart;
   prm.xend[p] = o.xend;
-  prm.ystart[p] = o.ystart;
+  if (!SCORES) prm.ystart[p] = o.ystart;
   prm.yend[p] = o.yend;
-  prm.n_ops[p] = o.n_ops;
-  prm.ops_src[p] = prm.ops_off[p] - o.n_ops;
+  if (!SCORES) {
+    prm.n_ops[p] = o.n_ops;
+    prm.ops_src[p] = prm.ops_off[p] - o.n_ops;
+  }
   prm.status[p] = o.status;
   if (o.status) atomicOr(prm.err_flag, o.status == 2 ? 2u : (o.status == 4 ? 8u : 1u));
-  for (int q = 0; q < 4; ++q) prm.clip_len[4 * p + q] = o.clip[q];
+  if (!SCORES)
+    for (int q = 0; q < 4; ++q) prm.clip_len[4 * p + q] = o.clip[q];
 }
 
 __global__ void __launch_bounds__(128, B2A_K3_MINB) banded_fill_kernel(const BandedParams prm, uint32_t n_wave) {
@@ -2777,6 +2797,20 @@ __global__ void __launch_bounds__(128, 8) banded_strip_finish_kernel(const Bande
 }
 __global__ void __launch_bounds__(128) banded_strip_walk_kernel(const BandedParams prm, uint32_t n_wave) {
   banded_fill_body<-1, 2, 1>(prm, n_wave);  // one pair per thread
+}
+// the score-only twins.  The strip path keeps its walk kernel (one pair per thread) after the finish pass: measured
+// against a finish pass that walks on lane 0 itself, it took slightly less K3 time (DESIGN.md §4)
+__global__ void __launch_bounds__(128, B2A_K3_MINB) banded_fill_scores_kernel(const BandedParams prm, uint32_t n_wave) {
+  banded_fill_body<0, 0, 32, true>(prm, n_wave);
+}
+__global__ void __launch_bounds__(128, 4) banded_fill_fast_scores_kernel(const BandedParams prm, uint32_t n_wave) {
+  banded_fill_body<K3_FAST_ROWS, 0, 32, true>(prm, n_wave);
+}
+__global__ void __launch_bounds__(128, 8) banded_strip_finish_scores_kernel(const BandedParams prm, uint32_t n_wave) {
+  banded_fill_body<-1, 1, 32, true>(prm, n_wave);
+}
+__global__ void __launch_bounds__(128) banded_strip_walk_scores_kernel(const BandedParams prm, uint32_t n_wave) {
+  banded_fill_body<-1, 2, 1, true>(prm, n_wave);  // one pair per thread
 }
 
 #endif

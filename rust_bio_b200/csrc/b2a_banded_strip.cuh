@@ -47,7 +47,8 @@ struct KsLayout {
   uint64_t tab, bnd, last, tb, total;
 };
 B2A_HD uint32_t ks_nstrips(uint64_t m) { return m >= 2 ? (uint32_t)((m - 1 + KS_ROWS - 1) / KS_ROWS) : 0u; }
-B2A_HD KsLayout ks_layout(uint64_t m, uint64_t band_cols, uint64_t strip_cols) {
+// score_only: the area of a score-only call (F_NOTB fill), without the traceback region
+B2A_HD KsLayout ks_layout(uint64_t m, uint64_t band_cols, uint64_t strip_cols, bool score_only = false) {
   KsLayout L;
   const uint64_t ns = ks_nstrips(m);
   uint64_t b = 0;
@@ -56,7 +57,7 @@ B2A_HD KsLayout ks_layout(uint64_t m, uint64_t band_cols, uint64_t strip_cols) {
   L.last = b; b = al16(b + (m + 1) * 8);  // column n-1's {4S, D} per row, when column n holds band cells
   L.tb = b;
   // a strip of `len` columns stores ceil((len + 14) / 8) groups of 8 steps, KS_TBW x KS_G uint4 each
-  b += (strip_cols / 8 + 3 * ns) * (uint64_t)(KS_TBW * KS_G * 16);
+  if (!score_only) b += (strip_cols / 8 + 3 * ns) * (uint64_t)(KS_TBW * KS_G * 16);
   L.total = (b + 255) & ~255ull;
   return L;
 }
@@ -151,6 +152,7 @@ B2A_HD void ks_column_step(const DevScoring& sc, const KsLut& T, const int32_t o
   constexpr bool CX = (FLAGS & F_CLIPX) != 0;
   constexpr bool CY = (FLAGS & F_CLIPY) != 0;
   constexpr bool LUT = (FLAGS & F_LUT) != 0;
+  constexpr bool NOTB = (FLAGS & F_NOTB) != 0;
   const int32_t go4i = 4 * sc.gap_open + 2, go4d = 4 * sc.gap_open + 1;
   const int32_t ma4 = 4 * sc.match_score + 3 - go4d, mi4 = 4 * sc.mismatch_score + 3 - go4d;
   const int32_t x4 = CX ? scale4(xclip_score(sc, j)) : NEG4;
@@ -172,8 +174,10 @@ B2A_HD void ks_column_step(const DevScoring& sc, const KsLut& T, const int32_t o
     else if (CY) sP = imax(sP, fmad(ge4, r, y4_first));
     else if (CX) sP = imax(sP, x4);
     s4 = sP & ~3;
-    const int32_t fi = addmin(i4, -iop, 4), fd = addmin(d4, -dop, 4);
-    tbacc[r] = (uint32_t)(fmad((int32_t)tbacc[r], k16, fmad(fd, k2, fi)) + sP - s4);
+    if (!NOTB) {
+      const int32_t fi = addmin(i4, -iop, 4), fd = addmin(d4, -dop, 4);
+      tbacc[r] = (uint32_t)(fmad((int32_t)tbacc[r], k16, fmad(fd, k2, fi)) + sP - s4);
+    }
     // Outside the band S is forced to the sentinel (what the reference reads there is MIN_SCORE).  I and D need no
     // forcing: a column's band rows are one run and so are a row's band columns (starts and ends never decrease), so
     // neither chain re-enters the band once it has left it -- above the band I derives from the sentinel top and a
@@ -237,6 +241,7 @@ B2A_HD void ks_run_strip(const KsPair& P, const DevScoring& sc, const KsLut& T, 
   constexpr bool TR = (FLAGS & F_TRACK_ROWS) != 0;
   constexpr bool TC = (FLAGS & F_TRACK_COLS) != 0;
   constexpr bool LUT = (FLAGS & F_LUT) != 0;
+  constexpr bool NOTB = (FLAGS & F_NOTB) != 0;  // score-only: no traceback (the strip table still records the windows)
   auto code_of = [&](uint8_t byte) -> int32_t {  // LUT code of a sequence byte; a byte outside the alphabet is flagged
     int32_t c = (int32_t)T.cmap[byte];
     if (c == 0xFF) {
@@ -264,8 +269,9 @@ B2A_HD void ks_run_strip(const KsPair& P, const DevScoring& sc, const KsLut& T, 
   jb = KS_SHFL(jb, 0);
   const int32_t len = (have && jb >= ja) ? jb - ja + 1 : 0;
   if (TR && len > 4095) redo = true;  // the packed row-tracker key holds a 12-bit column offset
-  const int32_t nsteps = (ks_warp_max(len > 0 ? len + KS_G - 1 : 0) + 7) & ~7;
-  const uint32_t K = len > 0 ? (uint32_t)((len + KS_G - 1 + 7) >> 3) : 0u;
+  // (NOTB: no groups of 8 steps to fill and store)
+  const int32_t nsteps = NOTB ? ks_warp_max(len > 0 ? len + KS_G - 1 : 0) : (ks_warp_max(len > 0 ? len + KS_G - 1 : 0) + 7) & ~7;
+  const uint32_t K = (len > 0 && !NOTB) ? (uint32_t)((len + KS_G - 1 + 7) >> 3) : 0u;
   uint4* tbs = P.tb + tb_used;
   if (have && l == 0) {
     P.tab[KS_TAB * s] = (uint32_t)ja;
@@ -362,14 +368,14 @@ B2A_HD void ks_run_strip(const KsPair& P, const DevScoring& sc, const KsLut& T, 
       in_s = sup;
       in_i = iup;
       in_tv = Tv;
-    } else {
+    } else if (!NOTB) {
 #pragma unroll
       for (int r = 0; r < KS_R; ++r) tbacc[r] <<= 4;
     }
     in_s = B2A_SHFL_UP(in_s, KS_G);
     in_i = B2A_SHFL_UP(in_i, KS_G);
     if (TC) in_tv = B2A_SHFL_UP(in_tv, KS_G);
-    if ((t & 7) == 7 && (uint32_t)(t >> 3) < K) {
+    if (!NOTB && (t & 7) == 7 && (uint32_t)(t >> 3) < K) {
       uint4* dst = tbs + (size_t)(t >> 3) * KS_TBW * KS_G + l;
 #pragma unroll
       for (int qd = 0; qd < KS_TBW; ++qd) {
@@ -448,7 +454,8 @@ B2A_HD void ks_run_task(const StripParams& prm, const KsLut& T, const uint32_t t
     const int32_t bc0 = (int32_t)prm.band_cols[3 * pair], bc1 = (int32_t)prm.band_cols[3 * pair + 1];
     P.c0 = imax(bc0, 1);
     P.c1 = imin(bc1, P.n - 1);
-    const KsLayout S = ks_layout((uint64_t)P.m, (uint64_t)(P.c1 >= P.c0 ? P.c1 - P.c0 + 1 : 0), prm.band_cols[3 * pair + 2]);
+    const KsLayout S = ks_layout((uint64_t)P.m, (uint64_t)(P.c1 >= P.c0 ? P.c1 - P.c0 + 1 : 0), prm.band_cols[3 * pair + 2],
+                                 (FLAGS & F_NOTB) != 0);
     uint8_t* area = prm.strip + prm.strip_off[t];
     P.tab = reinterpret_cast<uint32_t*>(area + S.tab);
     P.bnd = reinterpret_cast<int4*>(area + S.bnd);
@@ -460,9 +467,17 @@ B2A_HD void ks_run_task(const StripParams& prm, const KsLut& T, const uint32_t t
   int32_t prev_ja = 1, prev_jb = 0;
   uint32_t tb_used = 0;
   bool redo = false;
+  // F_NOTB twins with exactly three of the four trackers / prefix clips live and no LUT run the capturing form for every
+  // strip: one inlined copy of the strip loop instead of two.  Chosen by -Xptxas -v: with two copies three of these
+  // twins spill a few words more than their full kernels; with one copy for every twin, two others do, and the
+  // capture's three instructions per cell slow the common twins (semiglobal's K3 by 10 %).  Split this way no twin
+  // spills more than its full kernel (DESIGN.md §4).
+  constexpr int kLive = ((FLAGS & F_TRACK_ROWS) != 0) + ((FLAGS & F_TRACK_COLS) != 0) + ((FLAGS & F_CLIPX) != 0) +
+                        ((FLAGS & F_CLIPY) != 0);
+  constexpr bool kOneCopy = (FLAGS & F_NOTB) != 0 && (FLAGS & F_LUT) == 0 && kLive == 3;
   for (int32_t s = 0; s < ns_max; ++s) {
     // the capture of row m-1 costs three instructions per cell: only the warp's passes that hold a pair's last strip pay it
-    const bool any_last = ks_warp_max((P.m >= 2 && s == ns - 1) ? 1 : 0) != 0;
+    const bool any_last = kOneCopy || ks_warp_max((P.m >= 2 && s == ns - 1) ? 1 : 0) != 0;
     if (any_last) ks_run_strip<FLAGS, true>(P, prm.sc, T, prm.one, prm.ge4, lane, s, prev_ja, prev_jb, tb_used, redo);
     else ks_run_strip<FLAGS, false>(P, prm.sc, T, prm.one, prm.ge4, lane, s, prev_ja, prev_jb, tb_used, redo);
   }
@@ -505,6 +520,11 @@ __global__ void __launch_bounds__(KS_WARPS * 32, B2A_KS_MINB) banded_strip_fill_
     __syncwarp();
   }
 }
+
+// Launches the F_NOTB twin for `flags` (which include F_NOTB) on `st`.  The twins are instantiated in
+// b2a_banded_strip_notb.cu, a translation unit of their own, so that they compile beside b2a_engine.cu.
+// Returns cudaErrorInvalidValue for a flag set without a twin.
+cudaError_t launch_banded_strip_fill_notb(int flags, unsigned grid, size_t smem, cudaStream_t st, const StripParams& sp);
 
 #endif
 

@@ -1383,7 +1383,7 @@ int32_t b2a_align_batch_scores(b2a_engine* e, int32_t mode, const b2a_scoring* s
 
 static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, uint32_t k, uint32_t w,
                            const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
-                           b2a_stats* stats);
+                           b2a_stats* stats, bool score_only = false);
 
 // BitEnc storage as the input of Aligner::{custom,global,semiglobal,local} (and of the banded aligner when k > 0)
 static int32_t packed_view(b2a_engine* e, const b2a_packed_pairs* pp, b2a_pairs* view) {
@@ -1426,26 +1426,50 @@ int32_t b2a_align_batch_banded(b2a_engine* e, int32_t mode, const b2a_scoring* s
   return banded_impl(e, mode, s, k, w, pairs, nullptr, results, stats);
 }
 
-int32_t b2a_align_batch_banded_hinted(b2a_engine* e, int32_t mode, const b2a_scoring* s, uint32_t k, uint32_t w,
-                                      const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
-                                      b2a_stats* stats) {
-  if (!e || !hints) return B2A_E_INVALID;
+static int32_t check_band_hints(b2a_engine* e, const b2a_pairs* pairs, const b2a_band_hints* hints) {
   if (!hints->match_off || (!hints->match_xy && pairs && pairs->n_pairs && hints->match_off[pairs->n_pairs]))
     return e->fail(B2A_E_INVALID, "banded hints: match_off / match_xy missing");
   if (hints->path_off && (hints->allowed_mismatches >= 0 || hints->use_lcskpp_union))
     return e->fail(B2A_E_INVALID, "banded hints: a match path excludes allowed_mismatches / use_lcskpp_union");
+  return B2A_OK;
+}
+
+int32_t b2a_align_batch_banded_hinted(b2a_engine* e, int32_t mode, const b2a_scoring* s, uint32_t k, uint32_t w,
+                                      const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
+                                      b2a_stats* stats) {
+  if (!e || !hints) return B2A_E_INVALID;
+  const int32_t rc = check_band_hints(e, pairs, hints);
+  if (rc) return rc;
   return banded_impl(e, mode, s, k, w, pairs, hints, results, stats);
 }
 
+// score-only banded batch: b2a_align_batch_banded (hints == NULL) or b2a_align_batch_banded_hinted
+int32_t b2a_align_batch_banded_scores(b2a_engine* e, int32_t mode, const b2a_scoring* s, uint32_t k, uint32_t w,
+                                      const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
+                                      b2a_stats* stats) {
+  if (!e) return B2A_E_INVALID;
+  if (hints) {
+    const int32_t rc = check_band_hints(e, pairs, hints);
+    if (rc) return rc;
+  }
+  return banded_impl(e, mode, s, k, w, pairs, hints, results, stats, true);
+}
+
+// score_only: score, xend, yend and status only -- K3 slabs without interior cells, strip areas without traceback,
+// the score-only K3 / K3s kernels, no ops scratch and no ops compaction.  K4 and every path decision are the full call's.
 static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, uint32_t k, uint32_t w,
                            const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
-                           b2a_stats* stats) {
+                           b2a_stats* stats, bool score_only) {
   if (!e || !s || !pairs) return B2A_E_INVALID;
   if (k == 0) return e->fail(B2A_E_INVALID, "banded: k-mer length must be >= 1");
+  if (score_only && results && (results->xstart || results->ystart || results->ops || results->ops_off || results->clip_len))
+    return e->fail(B2A_E_INVALID, "a score-only batch has only score, xend, yend and status: xstart, ystart, ops, "
+                                  "ops_off and clip_len must be NULL");
   uint32_t maxm = 0, maxn = 0;
   int64_t score_bound = 0;
   int rc = stage_front(e, mode, s, pairs, maxm, maxn, score_bound);
   if (rc) return rc;
+  e->score_only = score_only;
   const uint64_t n = e->n_pairs;
   cudaStream_t st = e->stream;
   auto up = [&](DevBuf& bf, const void* src, size_t bytes) -> cudaError_t {
@@ -1453,12 +1477,13 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
     return bytes ? cudaMemcpyAsync(bf.p, src, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
   };
   // per-pair ops regions (written backwards from their end) and output arrays
-  std::vector<uint64_t> ops_end(n);
+  std::vector<uint64_t> ops_end(score_only ? 0 : n);
   uint64_t ops_total = 0;
-  for (uint64_t p = 0; p < n; ++p) {
-    ops_total += (uint64_t)pairs->x_len[p] + pairs->y_len[p] + 8;
-    ops_end[p] = ops_total;
-  }
+  if (!score_only)
+    for (uint64_t p = 0; p < n; ++p) {
+      ops_total += (uint64_t)pairs->x_len[p] + pairs->y_len[p] + 8;
+      ops_end[p] = ops_total;
+    }
   CK(e->d_xoff.reserve(n * 8 + 8));
   CK(e->d_yoff.reserve(n * 8 + 8));
   CK(e->d_xlen.reserve(n * 4 + 4));
@@ -1476,7 +1501,7 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
   CK(e->d_status.reserve(n * 4 + 4));
   CK(e->d_nops64.reserve((n + 1) * 8));
   CK(e->d_opsoff.reserve((n + 1) * 8));
-  CK(e->d_opsscratch.reserve(ops_total + 16));
+  if (!score_only) CK(e->d_opsscratch.reserve(ops_total + 16));
   CK(e->d_bcells.reserve(n * 8 + 8));
   CK(e->d_bstatus.reserve(n * 4 + 4));
   CK(e->d_bcols.reserve(n * 12 + 16));
@@ -1489,7 +1514,7 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
   }
   CK(up(e->d_codemap, e->codemap_host, 256));
   if (!e->lut_host.empty()) CK(up(e->d_lut, e->lut_host.data(), e->lut_host.size() * 4));
-  CK(up(e->d_bopsend, ops_end.data(), n * 8));
+  if (!score_only) CK(up(e->d_bopsend, ops_end.data(), n * 8));
   uint32_t* ctl = e->d_ctl.as<uint32_t>();
   CK(cudaMemsetAsync(ctl, 0, 256, st));
 
@@ -1591,7 +1616,7 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
   bp.clip_len = e->d_clip.as<uint32_t>();
   bp.status = e->d_status.as<uint32_t>();
   bp.err_flag = ctl + 1;
-  bp.ops_scratch = e->d_opsscratch.as<uint8_t>();
+  bp.ops_scratch = score_only ? nullptr : e->d_opsscratch.as<uint8_t>();
   bp.ops_off = e->d_bopsend.as<uint64_t>();
 
   e->launches = 0;
@@ -1667,10 +1692,10 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
         if (!(h_k4[t] & 0x200u)) return 0;
         const uint64_t mm = pairs->x_len[lo + t], nn = pairs->y_len[lo + t];
         const uint64_t c0 = std::max<uint64_t>(h_cols[3 * (size_t)t], 1), c1 = std::min<uint64_t>(h_cols[3 * (size_t)t + 1], nn - 1);
-        return ks_layout(mm, c1 >= c0 ? c1 - c0 + 1 : 0, h_cols[3 * (size_t)t + 2]).total;
+        return ks_layout(mm, c1 >= c0 ? c1 - c0 + 1 : 0, h_cols[3 * (size_t)t + 2], score_only).total;
       };
       while (s1 < nw) {
-        const uint64_t need = k3_slab_bytes(pairs->x_len[lo + s1], pairs->y_len[lo + s1], h_cells[s1]);
+        const uint64_t need = k3_slab_bytes(pairs->x_len[lo + s1], pairs->y_len[lo + s1], h_cells[s1], score_only);
         const uint64_t sneed = strip_need(s1);
         if (s1 > s0 && fbytes + sbytes + need + sneed > budget / 2) break;
         foff.push_back(fbytes);
@@ -1726,13 +1751,17 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
         sp.ge4 = 4 * e->sc.gap_extend;
         const int fl = (e->sc.yclip_suffix > DEAD_CLIP ? (int)F_TRACK_ROWS : 0) | (e->sc.xclip_suffix > DEAD_CLIP ? (int)F_TRACK_COLS : 0) |
                        (e->sc.xclip_prefix > DEAD_CLIP ? (int)F_CLIPX : 0) | (e->sc.yclip_prefix > DEAD_CLIP ? (int)F_CLIPY : 0) |
-                       (s->table ? (int)F_LUT : 0);
+                       (s->table ? (int)F_LUT : 0) | (score_only ? (int)F_NOTB : 0);
         sp.flags = fl;
         CK(cudaMemsetAsync(sp.task_counter, 0, 4, st));
         const uint32_t ntasks = (sp.n_elig + 3) / 4;
         const unsigned sgrid = (unsigned)std::min<uint32_t>((ntasks + KS_WARPS - 1) / KS_WARPS, (uint32_t)e->num_sms * (uint32_t)B2A_KS_MINB);
         const size_t ks_smem = ks_smem_bytes(fl, e->sc.alpha);
-        switch (fl) {
+        if (score_only) {  // the F_NOTB twins (b2a_banded_strip_notb.cu)
+          const cudaError_t ce = launch_banded_strip_fill_notb(fl, sgrid, ks_smem, st, sp);
+          if (ce == cudaErrorInvalidValue) return e->fail(B2A_E_INVALID, "banded strip fill: unexpected flag set");
+          CK(ce);
+        } else switch (fl) {
 #define B2A_KS_CASE1(F)                                                                                                   \
   case (F):                                                                                                               \
     if (ks_smem > 48 * 1024)                                                                                              \
@@ -1763,11 +1792,19 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
         CK(cudaGetLastError());
         b3.strip = sp.strip;
         b3.strip_off = sp.strip_off;
-        banded_strip_finish_kernel<<<(ns + 3) / 4, 128, 0, st>>>(b3, ns);
-        CK(cudaGetLastError());
-        banded_strip_walk_kernel<<<(ns + 127) / 128, 128, 0, st>>>(b3, ns);  // one pair per thread
-        CK(cudaGetLastError());
-        e->launches += 3;
+        if (score_only) {
+          banded_strip_finish_scores_kernel<<<(ns + 3) / 4, 128, 0, st>>>(b3, ns);
+          CK(cudaGetLastError());
+          banded_strip_walk_scores_kernel<<<(ns + 127) / 128, 128, 0, st>>>(b3, ns);  // one pair per thread
+          CK(cudaGetLastError());
+          e->launches += 3;
+        } else {
+          banded_strip_finish_kernel<<<(ns + 3) / 4, 128, 0, st>>>(b3, ns);
+          CK(cudaGetLastError());
+          banded_strip_walk_kernel<<<(ns + 127) / 128, 128, 0, st>>>(b3, ns);  // one pair per thread
+          CK(cudaGetLastError());
+          e->launches += 3;
+        }
         e->strip_pairs += elig.size();
       }
       // The column loops, one warp per pair, for the pairs K4 did not mark for the strip path (K4 marked those whose
@@ -1796,11 +1833,11 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
           CK(cudaStreamWaitEvent(st, e->sub_ev[3], 0));
         }
         if (e->banded_fast) {
-          banded_fill_fast_kernel<<<(ns + 3) / 4, 128, 0, ks>>>(bc, ns);
+          (score_only ? banded_fill_fast_scores_kernel : banded_fill_fast_kernel)<<<(ns + 3) / 4, 128, 0, ks>>>(bc, ns);
           CK(cudaGetLastError());
           ++e->launches;
         }
-        banded_fill_kernel<<<(ns + 3) / 4, 128, 0, ks>>>(bc, ns);
+        (score_only ? banded_fill_scores_kernel : banded_fill_kernel)<<<(ns + 3) / 4, 128, 0, ks>>>(bc, ns);
         CK(cudaGetLastError());
         ++e->launches;
       }
@@ -1814,8 +1851,10 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
     lo += nw;
   }
   CK(cudaEventRecord(e->ev[4], st));
-  rc = compact_ops(e, ops_total, st);
-  if (rc) return rc;
+  if (!score_only) {
+    rc = compact_ops(e, ops_total, st);
+    if (rc) return rc;
+  }
   CK(cudaEventRecord(e->ev[5], st));
   e->plan = Plan{};
   e->plan.cells = total_cells;

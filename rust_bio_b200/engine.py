@@ -233,8 +233,20 @@ class Engine:
                                   use_lcskpp_union: bool = False, results: Optional[Results] = None) -> Results:
         """banded::Aligner::custom_with_{matches, expanded_matches, match_path} over a batch
         (b2a_align_batch_banded_hinted): matches[p] = [(xpos, ypos), ...] per pair, paths[p] = [index, ...]."""
-        from ._lib import CBandHints
         n = len(batch[2])
+        h, keep = self._band_hints(n, matches, paths, allowed_mismatches, use_lcskpp_union)
+        if results is None:
+            results = Results(n, self.default_ops_capacity(batch))
+        cp = self._cpairs(batch)
+        self._check(self._L.b2a_align_batch_banded_hinted(self._h, int(mode), C.byref(cscoring), int(k), int(w),
+                                                          C.byref(cp), C.byref(h), C.byref(results.c),
+                                                          C.byref(self.stats)))
+        return results
+
+    @staticmethod
+    def _band_hints(n: int, matches, paths, allowed_mismatches, use_lcskpp_union):
+        """b2a_band_hints of per-pair match lists (and paths) -> (CBandHints, the arrays it points into)"""
+        from ._lib import CBandHints
         if len(matches) != n or (paths is not None and len(paths) != n):
             raise ValueError("one match list (and path) per pair")
         moff = np.zeros(n + 1, dtype=np.uint64)
@@ -244,18 +256,31 @@ class Engine:
             mxy = np.zeros(2, dtype=np.uint32)
         h = CBandHints(moff.ctypes.data, mxy.ctypes.data, None, None,
                        -1 if allowed_mismatches is None else int(allowed_mismatches), 1 if use_lcskpp_union else 0)
+        keep = [moff, mxy]
         if paths is not None:
             poff = np.zeros(n + 1, dtype=np.uint64)
             poff[1:] = np.cumsum([len(p) for p in paths])
             pidx = np.array([v for p in paths for v in p] or [0], dtype=np.uint32)
             h.path_off, h.path_idx = poff.ctypes.data, pidx.ctypes.data
-        if results is None:
-            results = Results(n, self.default_ops_capacity(batch))
+            keep += [poff, pidx]
+        return h, keep
+
+    def align_batch_banded_scores(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch, matches=None,
+                                  paths=None, allowed_mismatches: Optional[int] = None,
+                                  use_lcskpp_union: bool = False) -> Dict[str, np.ndarray]:
+        """b2a_align_batch_banded_scores: the banded aligner's Alignment.score / xend / yend without the traceback ->
+        {score, xend, yend, status} (numpy, caller's pair order).  matches (and paths, allowed_mismatches,
+        use_lcskpp_union) as in align_batch_banded_hinted; matches=None finds them on the device."""
+        n = len(batch[2])
+        h = keep = None
+        if matches is not None:
+            h, keep = self._band_hints(n, matches, paths, allowed_mismatches, use_lcskpp_union)
+        res = ScoreResults(n)
         cp = self._cpairs(batch)
-        self._check(self._L.b2a_align_batch_banded_hinted(self._h, int(mode), C.byref(cscoring), int(k), int(w),
-                                                          C.byref(cp), C.byref(h), C.byref(results.c),
-                                                          C.byref(self.stats)))
-        return results
+        self._check(self._L.b2a_align_batch_banded_scores(self._h, int(mode), C.byref(cscoring), int(k), int(w),
+                                                          C.byref(cp), C.byref(h) if h is not None else None,
+                                                          C.byref(res.c), C.byref(self.stats)))
+        return res.as_dict()
 
     def banded_band_ranges(self, pair: int, y_len: int) -> np.ndarray:
         """Band::ranges of `pair` of the last banded call: array [y_len + 1, 2] of (start, end) row ranges."""

@@ -177,6 +177,22 @@ def _alignments(res: Results, pairs, mode: int, on_panic: str, banded: bool = Fa
     return out
 
 
+def _alignment_scores(res, n: int, on_panic: str) -> list:
+    """{score, xend, yend, status} of a score-only call -> [AlignmentScore]; per-pair failures raise or become None
+    (as in _alignments)."""
+    from ._lib import B2AError
+    out = []
+    for i in range(n):
+        st = int(res["status"][i])
+        if st:
+            if on_panic == "raise":
+                raise B2AError(-4 if st == 1 else (-5 if st == 2 else -1), f"pair {i}: " + _PAIR_STATUS_TEXT.get(st, str(st)))
+            out.append(None)
+            continue
+        out.append(AlignmentScore(int(res["score"][i]), int(res["xend"][i]), int(res["yend"][i])))
+    return out
+
+
 def _check_scoring(s: Scoring):
     """Aligner::with_capacity_and_scoring asserts, mod.rs:554-571"""
     assert s.gap_open <= 0, "gap_open can't be positive"
@@ -250,20 +266,9 @@ class Aligner:
         """Alignment.score / xend / yend of each pair without the traceback (b2a_align_batch_scores): what the full
         call returns in those fields.  on_panic as in _batch; a panic only the traceback's interior would meet
         cannot be seen here, and such a pair reports its score (include/b200align.h)."""
-        from ._lib import B2AError
         batch = pack_pairs(pairs)
         cs, keep = self.scoring.to_c(batch)
-        res = self.engine.align_batch_scores(mode, cs, batch)
-        out = []
-        for i in range(len(pairs)):
-            st = int(res["status"][i])
-            if st:
-                if on_panic == "raise":
-                    raise B2AError(-4, f"pair {i}: " + _PAIR_STATUS_TEXT.get(st, str(st)))
-                out.append(None)
-                continue
-            out.append(AlignmentScore(int(res["score"][i]), int(res["xend"][i]), int(res["yend"][i])))
-        return out
+        return _alignment_scores(self.engine.align_batch_scores(mode, cs, batch), len(pairs), on_panic)
 
     def custom_scores_batch(self, pairs, on_panic: str = "raise") -> List[Optional["AlignmentScore"]]:
         return self._scores_batch(MODE_CUSTOM, pairs, on_panic)

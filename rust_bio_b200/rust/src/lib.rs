@@ -120,6 +120,17 @@ pub mod alignment {
                 results: *mut b2a_results,
                 stats: *mut c_void,
             ) -> i32;
+            fn b2a_align_batch_banded_scores(
+                e: *mut c_void,
+                mode: i32,
+                scoring: *const b2a_scoring,
+                k: u32,
+                w: u32,
+                pairs: *const b2a_pairs,
+                hints: *const b2a_band_hints,
+                results: *mut b2a_results,
+                stats: *mut c_void,
+            ) -> i32;
         }
         #[repr(C)]
         struct b2a_band_hints {
@@ -525,9 +536,10 @@ pub mod alignment {
             pub fn semiglobal_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { self.batch(2, None, pairs) }
             pub fn local_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { self.batch(3, None, pairs) }
 
-            /// Alignment::{score, xend, yend} of each pair without the traceback (b2a_align_batch_scores), on this
-            /// aligner's device.  Panics where the full call would (a pair the reference panics on).
-            pub(crate) fn scores_batch(&mut self, mode: i32, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> {
+            /// Alignment::{score, xend, yend} of each pair without the traceback (b2a_align_batch_scores, or with
+            /// banded = Some((k, w)) b2a_align_batch_banded_scores), on this aligner's device.  Panics where the full
+            /// call would (a pair the reference panics on).
+            pub(crate) fn scores_batch(&mut self, mode: i32, banded: Option<(u32, u32)>, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> {
                 let n = pairs.len();
                 let pb = self.pack(pairs);
                 let (cs, cp) = (self.c_scoring(&pb), pb.c_pairs());
@@ -545,7 +557,13 @@ pub mod alignment {
                     clip_len: std::ptr::null_mut(),
                     status: std::ptr::null_mut(),
                 };
-                let rc = unsafe { b2a_align_batch_scores(self.engine, mode, &cs, &cp, &mut res, std::ptr::null_mut()) };
+                let rc = match banded {
+                    None => unsafe { b2a_align_batch_scores(self.engine, mode, &cs, &cp, &mut res, std::ptr::null_mut()) },
+                    Some((k, w)) => unsafe {
+                        b2a_align_batch_banded_scores(self.engine, mode, &cs, k, w, &cp, std::ptr::null(), &mut res,
+                                                      std::ptr::null_mut())
+                    },
+                };
                 if rc != 0 {
                     let msg = unsafe { CStr::from_ptr(b2a_last_error(self.engine)) }.to_string_lossy().into_owned();
                     panic!("{}", msg);
@@ -553,10 +571,10 @@ pub mod alignment {
                 (0..n).map(|p| AlignmentScore { score: score[p], xend: xe[p] as usize, yend: ye[p] as usize }).collect()
             }
 
-            pub fn custom_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(0, pairs) }
-            pub fn global_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(1, pairs) }
-            pub fn semiglobal_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(2, pairs) }
-            pub fn local_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(3, pairs) }
+            pub fn custom_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(0, None, pairs) }
+            pub fn global_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(1, None, pairs) }
+            pub fn semiglobal_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(2, None, pairs) }
+            pub fn local_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { self.scores_batch(3, None, pairs) }
 
             /// mod.rs:591
             pub fn custom(&mut self, x: &[u8], y: &[u8]) -> Alignment { self.batch(0, None, &[(x, y)]).remove(0) }
@@ -610,7 +628,7 @@ pub mod alignment {
 
         // ------------------------------------------------------------ banded::Aligner, banded.rs:122-1004
         pub mod banded {
-            use super::{Alignment, BandedCall, MatchFunc, Scoring};
+            use super::{Alignment, AlignmentScore, BandedCall, MatchFunc, Scoring};
 
             /// Same constructors and methods as `bio::alignment::pairwise::banded::Aligner` (k = k-mer length,
             /// w = band half-width, banded.rs:150-267); every method is a batch of one, `*_batch` is the GPU form.
@@ -644,6 +662,12 @@ pub mod alignment {
                 pub fn global_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { let c = self.call(); self.inner.batch(1, Some(c), pairs) }
                 pub fn semiglobal_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { let c = self.call(); self.inner.batch(2, Some(c), pairs) }
                 pub fn local_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { let c = self.call(); self.inner.batch(3, Some(c), pairs) }
+                /// Alignment::{score, xend, yend} of each pair without the traceback (b2a_align_batch_banded_scores):
+                /// what the `*_batch` form returns in those fields; a band above MAX_CELLS gives (MIN_SCORE, 0, 0).
+                pub fn custom_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { let (k, w) = (self.k as u32, self.w as u32); self.inner.scores_batch(0, Some((k, w)), pairs) }
+                pub fn global_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { let (k, w) = (self.k as u32, self.w as u32); self.inner.scores_batch(1, Some((k, w)), pairs) }
+                pub fn semiglobal_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { let (k, w) = (self.k as u32, self.w as u32); self.inner.scores_batch(2, Some((k, w)), pairs) }
+                pub fn local_scores_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> { let (k, w) = (self.k as u32, self.w as u32); self.inner.scores_batch(3, Some((k, w)), pairs) }
                 /// banded.rs:282
                 pub fn custom(&mut self, x: &[u8], y: &[u8]) -> Alignment { self.custom_batch(&[(x, y)]).remove(0) }
                 /// banded.rs:872
