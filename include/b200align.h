@@ -68,7 +68,8 @@ enum {
   B2A_E_RANGE = -4,       /* scores/lengths would overflow i32 in the reference recurrence */
   B2A_E_CAPACITY = -5,    /* caller's ops buffer too small */
   B2A_E_STATE = -6,       /* stage/run/fetch called out of order */
-  B2A_E_UNSUPPORTED = -7  /* sequence too long for this build's on-chip staging */
+  B2A_E_UNSUPPORTED = -7  /* a forced fill shape that cannot stage the batch's sequences on chip, or one pair whose
+                             traceback alone exceeds the traceback budget (the score-only calls align it) */
 };
 
 /* Scoring<F> (mod.rs:238-247).  `table`, when non-NULL, is the host-tabulated
@@ -164,10 +165,15 @@ const char* b2a_version(void);
 /* Run all engine work on this cudaStream_t (default: an engine-owned stream). */
 int32_t b2a_engine_set_stream(b2a_engine* e, void* cuda_stream);
 /* Upper bound (bytes) on device scratch for traceback bit-vectors; larger
- * batches are processed in waves. 0 = default (60% of free HBM). */
+ * batches are processed in waves. 0 = default (60% of free HBM).  With the warp-per-pair shape a block holds fewer
+ * than 32 pairs when that keeps it within the budget, so waves can close between long pairs; a single pair whose
+ * traceback alone is above the budget is B2A_E_UNSUPPORTED before anything is allocated. */
 int32_t b2a_engine_set_traceback_budget(b2a_engine* e, uint64_t bytes);
 /* Force the fill-kernel shape (lanes per pair G in {1,2,4,8,32}, rows per
- * lane R in {8,16,20}: the built pairs are 1x8 1x16 1x20 2x16 2x20 4x16 8x16 8x20 32x8 32x16); 0,0 = automatic. */
+ * lane R in {8,16,20}: the built pairs are 1x8 1x16 1x20 2x16 2x20 4x16 8x16 8x20 32x8 32x16); 0,0 = automatic.
+ * The shapes with several pairs per warp stage whole sequences in shared memory: forced, a batch they cannot stage
+ * is B2A_E_UNSUPPORTED (the automatic choice falls back to the warp-per-pair shape).  32x8 and 32x16 stage one strip
+ * of x and read y from device memory: they take any length up to 2^24. */
 int32_t b2a_engine_set_tuning(b2a_engine* e, int32_t lanes_per_pair, int32_t rows_per_lane);
 
 /* The alphabet the last stage used: the caller's, or the byte values the engine found in the batch when

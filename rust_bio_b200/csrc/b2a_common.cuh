@@ -7,6 +7,7 @@
 // wavefront (b2a_fill.cuh), rows 1..m-1 only; row m, the last-column fix-ups and
 // the traceback walk run thread-per-pair in b2a_walk.cuh.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 #if defined(__CUDACC__)
@@ -86,6 +87,9 @@ enum : int {
                      // to fit a signed 16-bit half: 4*score_bound + 3 < 2^15 (boundary8_ok in b2a_plan.h)
   F_NOTB = 512,      // score-only batches: no interior traceback is accumulated or stored (the last column still writes
                      // its nibbles to ROWS_NL: K2's fix-ups and the edge walk read them)
+  F_YSTREAM = 1024,  // warp-per-pair shape (G == 32) when the batch's y does not fit its shared-memory staging: the task
+                     // stages only its strip of x, and each lane reads y from the staged-sequence arena one 32-bit
+                     // word ahead (whole-y staging is kept where y fits: it measured faster on C5)
 };
 #ifndef B2A_KREL_BITS
 #define B2A_KREL_BITS 12  // (a test build shortens the chunks to exercise the flushes on small inputs)
@@ -106,7 +110,7 @@ struct DevScoring {
 // one contiguous access.
 struct Block {
   uint32_t first;    // first sorted pair
-  uint32_t npairs;   // <= 32
+  uint32_t npairs;   // <= 32 (fewer in the last block, and in warp-per-pair blocks cut to the traceback budget)
   uint32_t maxm, maxn;
   uint32_t uniform;  // every pair of the block has m == maxm and n == maxn
   uint32_t nstrips;  // row strips of G*R rows covering rows 1..maxm-1
@@ -118,13 +122,22 @@ struct Block {
   uint64_t bnd_off;  // bytes into the boundary arena: (maxn+1) * 32 * 16, or (maxn+1) * 32 * 8 under F_BND8
   uint64_t rows_off; // bytes into the rows arena: 5 arrays of rows_pad*32 int32
   uint64_t rowm_off; // bytes into the row-m arena: (maxn+1)*32 bytes
-  uint64_t tb_off;   // bytes into the traceback arena: G * nstrips * K * TBW * 512
+  uint64_t tb_off;   // bytes into the traceback arena: G * nstrips * K * TBW * 512 (G == 32: npairs * ...)
   uint64_t ops_off;  // bytes into the ops scratch: 32 * (maxm+maxn+4)
   uint64_t strip_task_base;  // strip-pipelined fill (G == 32): tasks (pair, strip) of earlier blocks of the wave
+                             // (npairs * nstrips per block)
 };
 
 // rows arena sub-arrays (each rows_pad*32 int32, index [row][pair])
 enum { ROWS_SN = 0, ROWS_LY = 1, ROWS_SL = 2, ROWS_IL = 3, ROWS_NL = 4, ROWS_ARRAYS = 5 };
+
+// Element of the rows arena: array `arr`, slot = row * 32 + pair of a block.  64-bit: ROWS_ARRAYS * rows_pad * 32
+// passes 2^31 once m exceeds about 13.4 million (the engine takes m up to 2^24).  Only the array's base is widened:
+// arr * rows_pad and the slot both stay below 2^31, and the base is loop-invariant, so the kernels keep their 32-bit
+// slot arithmetic (an unsigned 32-bit offset, exact as well, made the warp-per-pair fill spill).
+B2A_HD int64_t rows_index(int arr, int32_t rows_pad, int32_t slot) {
+  return (int64_t)(arr * rows_pad) * 32 + slot;
+}
 
 B2A_HD int32_t imax(int32_t a, int32_t b) { return a > b ? a : b; }
 

@@ -623,10 +623,16 @@ static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* 
     if (!e->shape) return e->fail(B2A_E_INVALID, "no fill kernel for the requested shape");
     build_plan(e->plan, pairs->x_len, pairs->y_len, n, G, R, budget, e->flags);
     if (64 + lut_bytes + (uint64_t)fill_warps_of(G, R) * e->plan.smem_seq_bytes <= kMaxStageSmem) break;
+    if (G == 32) {
+      // the warp-per-pair shape stages one strip of x and y per warp; when y does not fit (n above ~50,000) it reads
+      // y from the staged-sequence arena instead (F_YSTREAM), so it takes any length
+      e->flags |= F_YSTREAM;
+      e->plan.smem_seq_bytes = (uint32_t)(G * R);
+      break;
+    }
     // Shapes with several pairs per warp stage 32/G whole (x, y) per warp; long sequences (a read against a
-    // 15 kb reference ...) only fit the warp-per-pair shape, which stages one strip of x and one y per warp
-    // (n up to ~50,000 symbols: 4 warps x (n + G*R + padding) bytes <= 200 KB).  Forced shapes are not replaced.
-    if ((e->tune_G && e->tune_R) || G == 32 || attempt > 0)
+    // 15 kb reference ...) take the warp-per-pair shape.  Forced shapes are not replaced.
+    if ((e->tune_G && e->tune_R) || attempt > 0)
       return e->fail(B2A_E_UNSUPPORTED, "sequences too long for on-chip staging with this fill shape");
     G = 32;
     const uint64_t rows = maxm > 1 ? maxm - 1 : 1;
@@ -637,6 +643,12 @@ static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* 
     return e->fail(B2A_E_UNSUPPORTED, "score-only batches run only the fill shapes the automatic choice picks (1x16, 8x16, "
                                       "8x20, 32x8, 32x16); the forced shape has no score-only fill kernel");
   const Plan& pl = e->plan;
+  // the warp-per-pair plan gives a pair whose traceback alone is above the budget a block of its own (b2a_plan.h)
+  if (!score_only && pl.G == 32 && pl.max_tb > budget)
+    return e->fail(B2A_E_UNSUPPORTED, "a pair's traceback needs " + std::to_string(pl.max_tb) +
+                                          " bytes, above the traceback budget of " + std::to_string(budget) +
+                                          " bytes; the score-only calls (b2a_align_batch_scores, b2a_batch_stage_scores) "
+                                          "align it without a traceback");
 
   // device memory
   CK(e->d_xoff.reserve(n * 8 + 8));

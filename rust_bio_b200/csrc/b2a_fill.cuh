@@ -18,7 +18,8 @@
 // kernel needs to finish row m.  Traceback is 4 bits per cell, eight columns
 // per 32-bit register, flushed with 128-bit stores that are contiguous across
 // the warp.  Sequences arrive in shared memory by cp.async.bulk (TMA bulk copy)
-// completing on an mbarrier; substitution scores come from MatchParams
+// completing on an mbarrier (the warp-per-pair shape copies its strip of x, and y too when it fits;
+// else (F_YSTREAM) it streams y from the staged-sequence arena word by word); substitution scores come from MatchParams
 // compare/select or from a compact LUT in shared memory.
 #pragma once
 #include "b2a_common.cuh"
@@ -52,7 +53,8 @@ struct LaneCtx {
   DevScoring sc;
   const int32_t* lut;    // LUT in shared memory (device) / host memory (sim)
   const uint32_t* xs;    // staged x words of the task: [w][P]
-  const uint32_t* ys;    // staged y words of the task: [w][P]
+  const uint32_t* ys;    // y words of the task: [w][P] staged in shared memory; F_YSTREAM: the pair's y in the
+                         // staged-sequence arena (HBM), read word by word as the lanes reach it (ld_yword)
   int32_t m, n;          // this lane's pair
   int32_t maxn;          // block maximum (loop bound shared by the warp)
   int32_t maxm;          // block maximum of m (uniform blocks: every valid pair's m)
@@ -177,6 +179,27 @@ B2A_HD T ld_boundary(const T* p, bool bypass_l1) {
   return *p;
 #endif
 }
+// Rows-arena element (array arr, slot = row * 32 + pair).  The warp-per-pair shape takes x up to 2^24, whose offsets
+// pass 2^31: it indexes in 64 bits (rows_index); the other shapes stage x whole in shared memory, so their offsets
+// stay far below 2^31 and keep the 32-bit arithmetic.
+template <int G>
+B2A_HD auto rows_at(int arr, int32_t rows_pad, int32_t slot) {
+  if constexpr (G == 32) return rows_index(arr, rows_pad, slot);
+  else return arr * rows_pad * 32 + slot;
+}
+// F_YSTREAM: word w of the pair's y, from the staged-sequence arena (read-only for the fill's lifetime)
+#ifndef B2A_HOST_YREAD
+#define B2A_HOST_YREAD(c, w) ((void)0)  // (tests/sim: checks every load against the pair's own words)
+#endif
+template <int G>
+B2A_HD uint32_t ld_yword(const LaneCtx<G>& c, int32_t w) {
+  B2A_HOST_YREAD(c, w);
+#if defined(__CUDA_ARCH__)
+  return __ldg(c.ys + w);
+#else
+  return c.ys[w];
+#endif
+}
 B2A_HD void fence_device() {
 #if defined(__CUDA_ARCH__)
   __threadfence();
@@ -287,9 +310,9 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
     }
     if (LAST) {
       const int32_t slot = (rowbase + 1 + r) * 32 + c.pi;
-      c.rows[ROWS_SL * c.rows_pad * 32 + slot] = s4 >> 2;
-      c.rows[ROWS_IL * c.rows_pad * 32 + slot] = i4 >> 2;
-      c.rows[ROWS_NL * c.rows_pad * 32 + slot] = nib;
+      c.rows[rows_at<G>(ROWS_SL, c.rows_pad, slot)] = s4 >> 2;
+      c.rows[rows_at<G>(ROWS_IL, c.rows_pad, slot)] = i4 >> 2;
+      c.rows[rows_at<G>(ROWS_NL, c.rows_pad, slot)] = nib;
     }
     if (MASKED && (CAPQ < 0 || (r >> 2) == CAPQ)) {
       if ((capbit >> r) & 1u) {
@@ -320,6 +343,8 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
   constexpr bool PK = (FLAGS & F_PACKTRK) != 0 || PR;  // packed keys in the lanes (PR: relative indices)
   constexpr bool B8 = (FLAGS & F_BND8) != 0;           // 8-byte boundary record (with F_PACKTRK only)
   constexpr bool NOTB = (FLAGS & F_NOTB) != 0;         // score-only: no traceback words (c.tb may be null)
+  constexpr bool YS = (FLAGS & F_YSTREAM) != 0;        // y read from the arena (warp-per-pair shape only)
+  static_assert(!YS || G == 32, "F_YSTREAM is a warp-per-pair form");
   static_assert(!B8 || ((FLAGS & F_PACKTRK) != 0 && !PR), "F_BND8 needs the packed column tracker with absolute rows");
   constexpr int P = 32 / G;
   constexpr int TBW = tbw_of(R);
@@ -384,9 +409,9 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       if (SnRr[r] != KEY_NONE) {
         const int32_t sn = (SnRr[r] >> 12) + ys;
         const int32_t step = (chunk << KREL_BITS) + (4095 - (SnRr[r] & 4095));
-        if (sn > c.rows[ROWS_SN * c.rows_pad * 32 + slot]) {
-          c.rows[ROWS_SN * c.rows_pad * 32 + slot] = sn;
-          c.rows[ROWS_LY * c.rows_pad * 32 + slot] = step - c.l + 1;  // the lane's column at that step
+        if (sn > c.rows[rows_at<G>(ROWS_SN, c.rows_pad, slot)]) {
+          c.rows[rows_at<G>(ROWS_SN, c.rows_pad, slot)] = sn;
+          c.rows[rows_at<G>(ROWS_LY, c.rows_pad, slot)] = step - c.l + 1;  // the lane's column at that step
         }
       }
       SnRr[r] = KEY_NONE;
@@ -418,6 +443,14 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       MASKED ? (rv >= 1 && (c.l == G - 1 || rowbase + R >= m - 1)) : (c.l == G - 1);
   int32_t cap_s = 0, cap_i = 0;
   uint32_t yw = 0;
+  // F_YSTREAM: the word of y after the current one, loaded four columns before it is needed; nothing past the pair's
+  // last word (ceil(n / 4)) is read, and a lane reads only on its active columns
+  int32_t nyw = 0;
+  uint32_t ynext = 0;
+  if constexpr (YS) {
+    nyw = (n + 3) >> 2;
+    if (nyw > 0) ynext = ld_yword(c, 0);
+  }
   uint4* tbs = NOTB ? nullptr : c.tb + (size_t)s * c.K * TBW * 32;
   const int32_t nsteps = c.K * 8;
 
@@ -425,8 +458,8 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       const int32_t slot = (rowbase + 1 + r) * 32 + c.pi;
-      c.rows[ROWS_SN * c.rows_pad * 32 + slot] = col0_S(c.sc, rowbase + 1 + r) + ys;  // column 0 (mod.rs:667-670)
-      c.rows[ROWS_LY * c.rows_pad * 32 + slot] = 0;
+      c.rows[rows_at<G>(ROWS_SN, c.rows_pad, slot)] = col0_S(c.sc, rowbase + 1 + r) + ys;  // column 0 (mod.rs:667-670)
+      c.rows[rows_at<G>(ROWS_LY, c.rows_pad, slot)] = 0;
       SnR[r] = KEY_NONE;
     }
   }
@@ -440,6 +473,14 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       int32_t q;
       if (G == 1) {
         if ((t & 3) == 0) yw = c.ys[(t >> 2) * P + c.g];
+        q = (int32_t)(yw & 0xffu);
+        yw >>= 8;
+      } else if (YS) {
+        if ((j & 3) == 1) {  // the first column of word (j - 1) / 4
+          yw = ynext;
+          const int32_t wn = ((j - 1) >> 2) + 1;
+          if (wn < nyw) ynext = ld_yword(c, wn);
+        }
         q = (int32_t)(yw & 0xffu);
         yw >>= 8;
       } else {
@@ -573,14 +614,17 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
         sn = (SnR[r] <= NEG4 / 2) ? MIN_SCORE : (SnR[r] >> 2);
         ly = LyR[r];
       }
-      c.rows[ROWS_SN * c.rows_pad * 32 + slot] = sn;
-      c.rows[ROWS_LY * c.rows_pad * 32 + slot] = ly;
+      c.rows[rows_at<G>(ROWS_SN, c.rows_pad, slot)] = sn;
+      c.rows[rows_at<G>(ROWS_LY, c.rows_pad, slot)] = ly;
     }
   }
 }
 
 template <int G, int R, int FLAGS>
 B2A_HD void fill_lane(const LaneCtx<G>& c) {
+  // warp-per-pair: the block's traceback has room for its real pairs only (b2a_plan.h), so a task of a padding pair
+  // (m = 0) stores nothing.  A real pair with m = 0 has no fill rows either: K2 reads none of its scratch.
+  if (G == 32 && c.m == 0) return;
   const int32_t s_lo = c.only_strip >= 0 ? c.only_strip : 0;
   const int32_t s_hi = c.only_strip >= 0 ? c.only_strip + 1 : c.nstrips;
   for (int32_t s = s_lo; s < s_hi; ++s) {
@@ -701,16 +745,18 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
     const Block blk = prm.blocks[b];
     if (strip_tasks && sub >= blk.npairs) continue;  // padding pair of the last block: nothing to do
     const uint32_t xbytes = blk.xwords * P * 4, ybytes = blk.ywords * P * 4;
-    // a strip task stages only the G*R x symbols of its own rows (P == 1 there); y is needed whole
+    // a strip task stages only the G*R x symbols of its own rows (P == 1 there); y is staged whole, or (F_YSTREAM)
+    // read from the arena by run_strip
     const uint32_t xoff = strip_tasks ? (uint32_t)only_strip * G * R : 0u;
     const uint32_t xstage = strip_tasks ? (uint32_t)(G * R) : xbytes;
+    constexpr bool YS = (FLAGS & F_YSTREAM) != 0;
     if (lane == 0) {
       // the previous task's generic-proxy reads of the staging buffer are done (syncwarp below)
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_expect_tx(bar, xstage + ybytes);
+      mbar_expect_tx(bar, xstage + (YS ? 0u : ybytes));
       const uint8_t* src = prm.seq + blk.seq_off;
       tma_bulk_g2s(stage, src + (size_t)sub * xbytes + xoff, xstage, bar);
-      tma_bulk_g2s(stage + xstage, src + (size_t)G * xbytes + (size_t)sub * ybytes, ybytes, bar);
+      if (!YS) tma_bulk_g2s(stage + xstage, src + (size_t)G * xbytes + (size_t)sub * ybytes, ybytes, bar);
     }
     LaneCtx<G> c;
     c.sc = prm.sc;
@@ -722,7 +768,8 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
     c.prog_mine = strip_tasks ? prm.progress + task : nullptr;
     c.prog_prev = (strip_tasks && only_strip > 0) ? prm.progress + task - 1 : nullptr;
     c.xs = reinterpret_cast<const uint32_t*>(stage) - xoff / 4;  // indexed by absolute row word
-    c.ys = reinterpret_cast<const uint32_t*>(stage + xstage);
+    c.ys = YS ? reinterpret_cast<const uint32_t*>(prm.seq + blk.seq_off + (size_t)G * xbytes + (size_t)sub * ybytes)
+              : reinterpret_cast<const uint32_t*>(stage + xstage);
     c.g = lane / G;
     c.l = lane % G;
     c.lane = lane;

@@ -58,8 +58,15 @@ cudaError_t B2A_CAT(B2A_LAUNCH_NAME, B2A_G, B2A_R)(int flags, const FillParams& 
 #else
   constexpr int NOTB = 0;
 #endif
+  // the warp-per-pair shape also has every case with y read from the arena (F_YSTREAM: y longer than its staging)
+#if B2A_G == 32
+#define B2A_CASE(F)                                                                    \
+  case (NOTB | (F)): return go<(NOTB | (F))>(prm, ntasks, num_sms, stream, grid_out, dry); \
+  case (NOTB | F_YSTREAM | (F)): return go<(NOTB | F_YSTREAM | (F))>(prm, ntasks, num_sms, stream, grid_out, dry);
+#else
 #define B2A_CASE(F) \
   case (NOTB | (F)): return go<(NOTB | (F))>(prm, ntasks, num_sms, stream, grid_out, dry);
+#endif
   switch (flags) {
     B2A_CASE(0)
     B2A_CASE(F_TRACK_ROWS)

@@ -1,4 +1,4 @@
-// Host-side batch plan: sort pairs by shape, cut them into blocks of 32, size
+// Host-side batch plan: sort pairs by shape, cut them into blocks of up to 32, size
 // the HBM arenas and the traceback waves.  Pure C++ (used by the engine and by
 // the CPU simulation harness in tests/sim/).
 #pragma once
@@ -37,7 +37,11 @@ inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 
 // `flags`: the fill's kernel flags (F_BND8 halves the boundary record; F_NOTB, a score-only batch, stores no
 // traceback, and its waves close on the rest of the per-wave scratch -- boundary rows, rows arena, row-m cells --
-// against the same budget)
+// against the same budget).
+// Blocks hold 32 pairs (the last one the rest), except in the warp-per-pair shape (G == 32) with a traceback: there a
+// block's traceback is sized by its real pairs, and a block closes early when its next pair would take it past
+// `tb_budget`, so that waves can close between long pairs.  A single pair above the budget still gets a block (and a
+// wave) of its own: the engine refuses such a batch (max_tb > tb_budget) before it allocates anything.
 inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, uint64_t n_pairs, int G,
                        int R, uint64_t tb_budget, int flags = 0) {
   const uint64_t bnd_rec = (flags & F_BND8) ? 8 : 16;
@@ -64,9 +68,31 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     p.pn[i] = y_len[p.order[i]];
     p.cells += (uint64_t)p.pm[i] * p.pn[i];
   }
-  const uint32_t nblocks = (uint32_t)((n_pairs + 31) / 32);
   const int P = 32 / G, TBW = tbw_of(R);
-  p.blocks.assign(nblocks, Block{});
+  // traceback bytes of one warp-task (32/G pairs) over every strip of a block with these maxima
+  auto task_tb = [&](uint32_t maxm, uint32_t maxn) -> uint64_t {
+    const uint64_t nstrips = maxm >= 2 ? (maxm - 1 + G * R - 1) / (G * R) : 0;
+    const uint64_t K = maxn ? (maxn + G - 1 + 7) / 8 : 0;
+    return nstrips * K * TBW * 512;
+  };
+  const bool per_pair = G == 32 && !notb;  // the warp-per-pair shape's tasks are its pairs
+  p.blocks.clear();
+  for (uint64_t first = 0; first < n_pairs;) {
+    uint32_t q = 0, mm = 0, mn = 0;
+    while (q < 32 && first + q < n_pairs) {
+      const uint32_t m2 = std::max(mm, p.pm[first + q]), n2 = std::max(mn, p.pn[first + q]);
+      if (per_pair && q > 0 && (uint64_t)(q + 1) * task_tb(m2, n2) > tb_budget) break;
+      mm = m2;
+      mn = n2;
+      ++q;
+    }
+    Block k{};
+    k.first = (uint32_t)first;
+    k.npairs = q;
+    p.blocks.push_back(k);
+    first += q;
+  }
+  const uint32_t nblocks = (uint32_t)p.blocks.size();
   p.waves.clear();
   p.seq_bytes = p.ops_bytes = 0;
   p.max_bnd = p.max_rows = p.max_rowm = p.max_tb = 0;
@@ -77,8 +103,6 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
   Wave w{0, 0, 0, 0, 0, 0, 0};
   for (uint32_t b = 0; b < nblocks; ++b) {
     Block& k = p.blocks[b];
-    k.first = b * 32;
-    k.npairs = (uint32_t)std::min<uint64_t>(32, n_pairs - (uint64_t)b * 32);
     k.maxm = k.maxn = 0;
     for (uint32_t q = 0; q < k.npairs; ++q) {
       k.maxm = std::max(k.maxm, p.pm[k.first + q]);
@@ -95,13 +119,15 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     k.rows_pad = k.nstrips * G * R + 2;
     p.maxm = std::max(p.maxm, k.maxm);
     p.maxn = std::max(p.maxn, k.maxn);
-    // the warp-per-pair shape runs (pair, strip) tasks that stage one strip of x (b2a_fill.cuh)
+    // the warp-per-pair shape runs (pair, strip) tasks that stage one strip of x (b2a_fill.cuh), and y unless the
+    // engine picks F_YSTREAM (y read from the arena: G * R bytes of staging)
     const uint32_t stage_x = G == 32 ? (uint32_t)(G * R) : k.xwords * P * 4;
     p.smem_seq_bytes = std::max<uint32_t>(p.smem_seq_bytes, stage_x + k.ywords * P * 4);
     const uint64_t bnd = align_up((uint64_t)(k.maxn + 1) * 32 * bnd_rec, 256);
     const uint64_t rows = align_up((uint64_t)ROWS_ARRAYS * k.rows_pad * 32 * 4, 256);
     const uint64_t rowm = align_up((uint64_t)(k.maxn + 1) * 32 * 2, 256);
-    const uint64_t tb = notb ? 0 : align_up((uint64_t)G * k.nstrips * k.K * TBW * 512, 256);
+    const uint32_t tasks = G == 32 ? k.npairs : (uint32_t)G;  // warp-tasks that store a traceback
+    const uint64_t tb = notb ? 0 : align_up((uint64_t)tasks * k.nstrips * k.K * TBW * 512, 256);
     const bool full = notb ? w.bnd_bytes + w.rows_bytes + w.rowm_bytes + bnd + rows + rowm > tb_budget
                            : w.tb_bytes + tb > tb_budget;
     if (b > w.block_lo && full) {  // close the wave
@@ -114,7 +140,7 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     k.ops_off = p.ops_bytes;
     p.ops_bytes += align_up((uint64_t)32 * (k.maxm + k.maxn + 4), 256);
     k.strip_task_base = w.strip_tasks;
-    w.strip_tasks += (uint64_t)32 * k.nstrips;
+    w.strip_tasks += (uint64_t)(G == 32 ? k.npairs : 32) * k.nstrips;
     k.bnd_off = w.bnd_bytes;
     k.rows_off = w.rows_bytes;
     k.rowm_off = w.rowm_bytes;
@@ -123,7 +149,7 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     w.rows_bytes += rows;
     w.rowm_bytes += rowm;
     w.tb_bytes += tb;
-    if (!notb) p.total_tb += (uint64_t)G * k.nstrips * k.K * TBW * 512;
+    if (!notb) p.total_tb += (uint64_t)tasks * k.nstrips * k.K * TBW * 512;
   }
   if (nblocks) {
     w.block_hi = nblocks;

@@ -105,7 +105,7 @@ struct PairView {
     if (sc.alpha) return lut[p * sc.alpha + q];
     return p == q ? sc.match_score : sc.mismatch_score;
   }
-  B2A_HD int32_t& row(int arr, int32_t i) const { return rows[(arr * rows_pad + i) * 32 + pi]; }
+  B2A_HD int32_t& row(int arr, int32_t i) const { return rows[rows_index(arr, rows_pad, i * 32 + pi)]; }
   // the record of column j as stored (decode_boundary); bnd8: the 8-byte record in x, y (z = w = 0)
   B2A_HD int4 load_bnd(int32_t j) const {
     const int64_t k = bnd_base + (int64_t)j * bnd_stride;
