@@ -5,7 +5,8 @@
 //   Aligner::custom   591-922   (cell rule 729-805, fix-ups 809-843, walk 845-908)
 // Nothing here is a translation of that loop nest: the fill is a row-strip
 // wavefront (b2a_fill.cuh), rows 1..m-1 only; row m, the last-column fix-ups and
-// the traceback walk run thread-per-pair in b2a_walk.cuh.
+// the traceback walk run thread-per-pair in b2a_walk.cuh (the thread-per-pair fill does row m and the fix-ups itself
+// under F_FINISH).
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -90,7 +91,13 @@ enum : int {
   F_YSTREAM = 1024,  // warp-per-pair shape (G == 32) when the batch's y does not fit its shared-memory staging: the task
                      // stages only its strip of x, and each lane reads y from the staged-sequence arena one 32-bit
                      // word ahead (whole-y staging is kept where y fits: it measured faster on C5)
+  F_FINISH = 2048,   // thread-per-pair fill (G == 1) without F_PACKREL: the lane also computes row m, the literal cells of
+                     // column n and both last-column fix-ups, and leaves each pair's EndState in the finish region
+                     // (FIN_* below) instead of S, I and the row trackers of column n in the rows arena (DESIGN.md §2)
 };
+// The finish region of an F_FINISH fill: FIN_FIELDS int32 per pair, [field][32] per block, blocks in wave order: the
+// EndState K2 reads (b2a_walk.cuh).
+enum { FIN_SMN = 0, FIN_IMN, FIN_CMN, FIN_SNM, FIN_LYM, FIN_LX0, FIN_LXN, FIN_FIELDS };
 #ifndef B2A_KREL_BITS
 #define B2A_KREL_BITS 12  // (a test build shortens the chunks to exercise the flushes on small inputs)
 #endif

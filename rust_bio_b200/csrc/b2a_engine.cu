@@ -140,7 +140,7 @@ struct b2a_engine {
   uint8_t codemap_host[256];
 
   DevBuf d_blob, d_xoff, d_xlen, d_yoff, d_ylen, d_order, d_pm, d_pn, d_blocks, d_seq, d_bnd, d_rows,
-      d_rowm, d_tb, d_opsscratch, d_lut, d_codemap, d_ctl, d_score, d_xs, d_xe, d_ys, d_ye, d_nops,
+      d_rowm, d_fin, d_tb, d_opsscratch, d_lut, d_codemap, d_ctl, d_score, d_xs, d_xe, d_ys, d_ye, d_nops,
       d_opssrc, d_clip, d_status, d_nops64, d_opsoff, d_opsdense, d_scan, d_records, d_prog, d_bcells, d_bstatus,
       d_bopsend, d_bslab, d_branges, d_broff, d_bfill, d_bfoff, d_hmoff, d_hmxy, d_hpoff, d_hpidx, d_raw, d_gnops,
       d_gnops64, d_goff, d_bcols, d_bstrip, d_bsoff, d_belig;
@@ -327,7 +327,7 @@ int32_t b2a_engine_destroy(b2a_engine* e) {
   if (e->h_plan) cudaFreeHost(e->h_plan);
   if (e->h_nops) cudaFreeHost(e->h_nops);
   DevBuf* bufs[] = {&e->d_blob, &e->d_xoff, &e->d_xlen, &e->d_yoff, &e->d_ylen, &e->d_order, &e->d_pm,
-                    &e->d_pn, &e->d_blocks, &e->d_seq, &e->d_bnd, &e->d_rows, &e->d_rowm, &e->d_tb,
+                    &e->d_pn, &e->d_blocks, &e->d_seq, &e->d_bnd, &e->d_rows, &e->d_rowm, &e->d_fin, &e->d_tb,
                     &e->d_opsscratch, &e->d_lut, &e->d_codemap, &e->d_ctl, &e->d_score, &e->d_xs,
                     &e->d_xe, &e->d_ys, &e->d_ye, &e->d_nops, &e->d_opssrc, &e->d_clip, &e->d_status,
                     &e->d_nops64, &e->d_opsoff, &e->d_opsdense, &e->d_scan, &e->d_records, &e->d_prog, &e->d_bcells,
@@ -561,6 +561,9 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
   return B2A_OK;
 }
 
+// the finish region of a launch whose blocks start `lo` blocks into the wave (F_FINISH; null stays null)
+static int32_t* fin_from(int32_t* fin, uint32_t lo) { return fin ? fin + (size_t)lo * FIN_FIELDS * 32 : nullptr; }
+
 // ops compaction shared by the full and the banded path: widen -> exclusive scan -> gather
 static int32_t compact_ops(b2a_engine* e, uint64_t scratch_bytes, cudaStream_t st) {
   const uint64_t n = e->n_pairs;
@@ -621,6 +624,11 @@ static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* 
   for (int attempt = 0;; ++attempt) {
     e->shape = find_shape(G, R);
     if (!e->shape) return e->fail(B2A_E_INVALID, "no fill kernel for the requested shape");
+    // the thread-per-pair fill finishes each pair's matrix itself (row m, column n, both fix-ups: F_FINISH), except
+    // with the relative packed trackers, whose row trackers are final only after the last chunk's flush; the
+    // launchers of that shape have no unfinished form
+    if (G == 1 && !(e->flags & F_PACKREL)) e->flags |= F_FINISH;
+    else e->flags &= ~F_FINISH;
     build_plan(e->plan, pairs->x_len, pairs->y_len, n, G, R, budget, e->flags);
     if (64 + lut_bytes + (uint64_t)fill_warps_of(G, R) * e->plan.smem_seq_bytes <= kMaxStageSmem) break;
     if (G == 32) {
@@ -663,6 +671,7 @@ static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* 
   CK(e->d_bnd.reserve(pl.max_bnd + 16));
   CK(e->d_rows.reserve(pl.max_rows + 16));
   CK(e->d_rowm.reserve(pl.max_rowm + 16));
+  CK(e->d_fin.reserve(pl.max_fin + 16));
   CK(e->d_tb.reserve(pl.max_tb + 16));
   CK(e->d_prog.reserve(pl.max_strip_tasks * 4 + 16));
   CK(e->d_opsscratch.reserve(pl.ops_bytes + 16));
@@ -778,6 +787,8 @@ int32_t b2a_batch_run(b2a_engine* e) {
     fp.bnd = e->d_bnd.as<uint8_t>();
     fp.rows = e->d_rows.as<uint8_t>();
     fp.tb = e->score_only ? nullptr : e->d_tb.as<uint8_t>();
+    fp.rowm = e->d_rowm.as<uint8_t>();
+    fp.fin = (e->flags & F_FINISH) ? e->d_fin.as<int32_t>() : nullptr;
     fp.lut = e->d_lut.as<int32_t>() + (size_t)e->sc.alpha * e->sc.alpha;  // the scaled copy
     fp.task_counter = ctl + 2 + wi;
     fp.smem_seq_bytes = pl.smem_seq_bytes;
@@ -817,6 +828,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     wp.R = pl.R;
     wp.packtrk = (e->flags & F_PACKTRK) ? 1 : 0;
     wp.bnd8 = (e->flags & F_BND8) ? 1 : 0;
+    wp.fin = fp.fin;
     wp.filter_clips = (e->mode == B2A_MODE_SEMIGLOBAL || e->mode == B2A_MODE_LOCAL) ? 1 : 0;
     wp.score = e->d_score.as<int32_t>();
     wp.xstart = e->d_xs.as<uint32_t>();
@@ -892,11 +904,13 @@ int32_t b2a_batch_run(b2a_engine* e) {
       fa.nblocks = split_b;
       fb.blocks = fp.blocks + split_b;
       fb.nblocks = nb - split_b;
+      fb.fin = fin_from(fp.fin, split_b);
       fb.task_counter = ctl + 8;
       WalkParams wa = wp, wb = wp;
       wa.nblocks = split_b;
       wb.blocks = wp.blocks + split_b;
       wb.nblocks = nb - split_b;
+      wb.fin = fb.fin;
       if (e->split_timing && !e->split_ev[0])
         for (auto& v : e->split_ev) CK(cudaEventCreate(&v));
       if (e->split_timing) CK(cudaEventRecord(e->split_ev[0], st));
@@ -953,6 +967,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
         FillParams f2 = fp;
         f2.blocks = fp.blocks + lo_b;
         f2.nblocks = hi_b - lo_b;
+        f2.fin = fin_from(fp.fin, lo_b);
         f2.task_counter = ctl + 8 + sidx;
         f2.task_limit = 1;  // CTAs retire after one task per warp: the walks' CTAs get onto the SMs in between
         CK(fill(e->flags, f2, f2.nblocks * (uint32_t)pl.G, e->num_sms, fs, &e->last_grid, 0));
@@ -963,6 +978,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
         WalkParams w2 = wp;
         w2.blocks = wp.blocks + lo_b;
         w2.nblocks = hi_b - lo_b;
+        w2.fin = f2.fin;
         if (warp_walk) walk_warp_k<<<w2.nblocks * 32 / wcta_warps, wcta_warps * 32, (size_t)per_warp_smem * wcta_warps, e->tail_stream>>>(w2);
         else walk_lane_k<<<(w2.nblocks * 32 + 127) / 128, 128, 0, e->tail_stream>>>(w2);
         CK(cudaGetLastError());

@@ -21,8 +21,13 @@
 // completing on an mbarrier (the warp-per-pair shape copies its strip of x, and y too when it fits;
 // else (F_YSTREAM) it streams y from the staged-sequence arena word by word); substitution scores come from MatchParams
 // compare/select or from a compact LUT in shared memory.
+// F_FINISH (thread-per-pair shape): the lane that fills a pair also finishes its matrix -- row m in the strip that
+// holds row m-1, and the literal cells of column n with both last-column fix-ups in each strip's last column, carried
+// from strip to strip in registers -- and leaves each pair's EndState in the finish region, so K2 only walks
+// (DESIGN.md §2).
 #pragma once
 #include "b2a_common.cuh"
+#include "b2a_walk.cuh"  // the row-m cell, the u16 cell helpers and the boundary decode (F_FINISH)
 
 namespace b2a {
 
@@ -35,6 +40,8 @@ struct FillParams {
   uint8_t* bnd;
   uint8_t* rows;
   uint8_t* tb;
+  uint8_t* rowm;       // F_FINISH: the row-m arena (u16 cells, as K2 writes them)
+  int32_t* fin;        // F_FINISH: the finish region, FIN_FIELDS * 32 int32 per block of the wave (else null)
   const int32_t* lut;  // scaled LUT 4*score + 3 - (4*gap_open + 1), alpha*alpha (global) or null
   uint32_t* task_counter;
   uint32_t smem_seq_bytes;  // per-warp staging bytes
@@ -75,7 +82,19 @@ struct LaneCtx {
   int32_t only_strip;    // strip-pipelined: the one strip this task fills (-1: all strips in order)
   int32_t one;           // an opaque 1 (kernel parameter): lets adds be issued as IMAD on the FMA pipe
   int32_t ge4;           // 4 * gap_extend, opaque as well (kept out of constant folding)
+  uint16_t* rowm = nullptr;  // F_FINISH: block base of the row-m arena, [column][32]
+  int32_t* fin = nullptr;    // F_FINISH: block base of the finish region, [field][32]
 };
+
+// F_FINISH: column n as the lane goes down it, row after row and strip after strip (held in registers)
+struct ColN {
+  int32_t S2;      // S(i-1, n) after both fix-ups
+  uint32_t c2;     // cell (i-1, n) after both fix-ups
+  uint32_t sp;     // s_bits(i-1, n) BEFORE the fix-ups: the i_bits of a cell whose I came from S of the row above
+  int32_t va, ia;  // fix-up 1 (mod.rs:809-821): the first row with the largest S + xs over rows 0..i-1
+  int32_t vb, ib;  // fix-up 2 (mod.rs:825-843): the first raised row with the largest S + xs (INT32_MIN: none yet)
+};
+
 
 #if defined(__CUDA_ARCH__)
 #define B2A_SHFL_UP(v, G) __shfl_up_sync(0xffffffffu, (v), 1, (G))
@@ -225,7 +244,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
                         const int32_t rv, int32_t (&Sp)[R], int32_t (&Dp)[R], int32_t (&SnR)[R],
                         int32_t (&LyR)[R], uint32_t (&tbacc)[R], const int32_t (&xc)[R],
                         int32_t sdiag, int32_t& sup, int32_t& iup, int32_t& Tv, int32_t& Ti,
-                        int32_t& cap_s, int32_t& cap_i) {
+                        int32_t& cap_s, int32_t& cap_i, ColN& cn) {
   constexpr bool TR = (FLAGS & F_TRACK_ROWS) != 0;
   constexpr bool TC = (FLAGS & F_TRACK_COLS) != 0;
   constexpr bool CX = (FLAGS & F_CLIPX) != 0;
@@ -234,6 +253,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
   constexpr bool PK = (FLAGS & F_PACKTRK) != 0 || PR;  // the caller passes chunk- / strip-relative cj and rowbase
   constexpr bool RELU = (FLAGS & F_RELU) != 0;
   constexpr bool NOTB = (FLAGS & F_NOTB) != 0;
+  constexpr bool FIN = (FLAGS & F_FINISH) != 0;
   constexpr bool TMASK = MASKED && !LUT;  // the column tracker has to skip the padded rows explicitly
   // S travels between cells as "S + open": So_d = S4 + go4d feeds the D chain of the next column and (as
   // the diagonal input) M of the next column, whose LUT/compare scores are pre-biased by -go4d; the I chain
@@ -249,6 +269,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
   const int32_t cj = 4095 - (PR ? (tstep & KREL_MASK) : j);
   const int32_t one = c.one, k2 = one + one, k16 = k2 * 8, k1024 = k16 * 64;
   const int32_t q4 = q * 4;
+  const int32_t qrow = LUT ? (int32_t)(c.lut_base + (uint32_t)(q * c.sc.alpha * 4)) : q;  // (F_FINISH, column n only)
   const uint32_t capbit = (MASKED && rv >= 1) ? 1u << (rv - 1) : 0u;  // one-hot: the lane's row m-1
   int32_t Tl = KEY_NONE;        // packed column tracker of this lane's rows (local row index)
   int32_t key_even = KEY_NONE;
@@ -310,9 +331,43 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
     }
     if (LAST) {
       const int32_t slot = (rowbase + 1 + r) * 32 + c.pi;
-      c.rows[rows_at<G>(ROWS_SL, c.rows_pad, slot)] = s4 >> 2;
-      c.rows[rows_at<G>(ROWS_IL, c.rows_pad, slot)] = i4 >> 2;
-      c.rows[rows_at<G>(ROWS_NL, c.rows_pad, slot)] = nib;
+      if (!FIN) {
+        c.rows[rows_at<G>(ROWS_SL, c.rows_pad, slot)] = s4 >> 2;
+        c.rows[rows_at<G>(ROWS_IL, c.rows_pad, slot)] = i4 >> 2;
+        c.rows[rows_at<G>(ROWS_NL, c.rows_pad, slot)] = nib;
+      } else if (!MASKED || r < rv) {
+        // cell (i, n), then fix-up 1 and fix-up 2 on it, as K2's passes would do them for this row (mod.rs:809-843)
+        const int32_t i = rowbase + 1 + r;
+        const uint32_t scode = (nib & 3) == NB_DIAG ? ((LUT ? xc[r] == qrow : xc[r] == q) ? TB_MATCH : TB_SUBST)
+                                                    : nib_scode_other((uint32_t)nib);
+        uint32_t cell = cell_make((nib & NB_IEXT) ? (uint32_t)TB_INS : cn.sp, (nib & NB_DEXT) ? (uint32_t)TB_DEL : LAZY, scode);
+        cn.sp = scode;
+        int32_t S = s4 >> 2;
+        int32_t Sn = MIN_SCORE;  // a dead yclip_suffix never wins (K2 does not read the row trackers then)
+        if (TR && c.sc.yclip_suffix > DEAD_CLIP) Sn = PK ? (SnR[r] >> 12) + c.sc.yclip_suffix
+                                                         : ((SnR[r] <= NEG4 / 2) ? MIN_SCORE : (SnR[r] >> 2));
+        if (Sn > S) {  // fix-up 1
+          S = Sn;
+          cell = cell_set_s(cell, TB_YCLIP_SUFFIX);
+        }
+        if (S + c.sc.xclip_suffix > cn.va) {
+          cn.va = S + c.sc.xclip_suffix;
+          cn.ia = i;
+        }
+        const int32_t s_score = cn.S2 + c.sc.gap_open;  // fix-up 2
+        if (s_score > (i4 >> 2)) cell = cell_set_i(cell, cell_s(cn.c2));
+        if (s_score > S) {
+          S = s_score;
+          cell = cell_set_s(cell, TB_INS);
+          if (S + c.sc.xclip_suffix > cn.vb) {
+            cn.vb = S + c.sc.xclip_suffix;
+            cn.ib = i;
+          }
+        }
+        cn.S2 = S;
+        cn.c2 = cell;
+        c.rows[rows_at<G>(ROWS_NL, c.rows_pad, slot)] = (int32_t)cell;
+      }
     }
     if (MASKED && (CAPQ < 0 || (r >> 2) == CAPQ)) {
       if ((capbit >> r) & 1u) {
@@ -333,9 +388,156 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
   }
 }
 
+// F_FINISH, before the last column of strip 0: column n starts with row 0 (mod.rs:698-714, fix-up 1 with
+// Sn[0] = yclip_suffix; its cell is written as it stays).  The lane then carries column n in registers down the strips.
+template <int G>
+B2A_HD void fin_column_n_begin(const LaneCtx<G>& c, ColN& cn) {
+  const DevScoring& sc = c.sc;
+  const int32_t n = c.n;
+  {
+    uint32_t c0 = cell_make(TB_START, row0_dbits(sc, n), row0_sbits(sc, n, n));
+    cn.sp = cell_s(c0);
+    int32_t S = row0_S(sc, n, n);
+    if (sc.yclip_suffix > S) {
+      S = sc.yclip_suffix;
+      c0 = cell_set_s(c0, TB_YCLIP_SUFFIX);
+    }
+    c.rows[rows_at<G>(ROWS_NL, c.rows_pad, c.pi)] = (int32_t)c0;
+    cn.S2 = S;
+    cn.c2 = c0;
+    cn.va = S + sc.xclip_suffix;
+    cn.ia = 0;
+    cn.vb = (int32_t)0x80000000;
+    cn.ib = 0;
+  }
+}
+// F_FINISH, column n of the strip holding row m-1 done and cell (m, n) made: the pair's EndState.  The x-suffix
+// tracker runs in the reference's order -- fix-up 1 over rows 0..m-1, then the Sn[m] test at i == m, then fix-up 2
+// in row order, each a strict '>' against the running S(m, n) -- so the two per-pass trackers are merged in that
+// order here (interleaving them per row would let a fix-up-2 raise take a tie from a later fix-up-1 row), and the
+// i == m step of fix-up 2 runs against the merged value (DESIGN.md §2).
+template <int G>
+B2A_HD void fin_end_state(const LaneCtx<G>& c, const ColN& cn, const RowM& rm, int32_t ImN, uint32_t cmN,
+                          const int32_t Lx0, int32_t LxN) {
+  const int32_t m = c.m;
+  int32_t SmN = rm.Sm;
+  if (cn.va > SmN) {  // fix-up 1
+    SmN = cn.va;
+    LxN = m - cn.ia;
+    cmN = cell_set_s(cmN, TB_XCLIP_SUFFIX);
+  }
+  if (rm.Snm > SmN) {  // i == m
+    SmN = rm.Snm;
+    cmN = cell_set_s(cmN, TB_YCLIP_SUFFIX);
+  }
+  if (cn.vb > SmN) {  // fix-up 2, rows 1..m-1
+    SmN = cn.vb;
+    LxN = m - cn.ib;
+    cmN = cell_set_s(cmN, TB_XCLIP_SUFFIX);
+  }
+  const int32_t s_score = cn.S2 + c.sc.gap_open;  // fix-up 2, i == m
+  if (s_score > ImN) {
+    ImN = s_score;
+    cmN = cell_set_i(cmN, cell_s(cn.c2));
+  }
+  if (s_score > SmN) {
+    SmN = s_score;
+    cmN = cell_set_s(cmN, TB_INS);
+  }
+  int32_t* f = c.fin + c.pi;
+  f[FIN_SMN * 32] = SmN;
+  f[FIN_IMN * 32] = ImN;
+  f[FIN_CMN * 32] = (int32_t)cmN;
+  f[FIN_SNM * 32] = rm.Snm;
+  f[FIN_LYM * 32] = rm.Lym;
+  f[FIN_LX0 * 32] = Lx0;
+  f[FIN_LXN * 32] = LxN;
+}
+
+// F_FINISH, right after the strip that holds row m-1: row m (mod.rs:641-645, 729-805 at i == m) with rowm_cell, K2's
+// rule, over the boundary records of row m-1 this lane has just stored (S, I and the column tracker, as K2 decoded
+// them; read back with plain loads, L2-resident: the lane wrote them itself), then the EndState.  Run inside the
+// strip's column loop instead, the row's carries pushed the C2 variant past its 168 registers into spills (DESIGN.md
+// §4).
+template <int G, int FLAGS>
+B2A_HD void fin_row_m(const LaneCtx<G>& c, const ColN& cn) {
+  constexpr bool LUT = (FLAGS & F_LUT) != 0;
+  constexpr bool PK = (FLAGS & F_PACKTRK) != 0;
+  constexpr bool B8 = (FLAGS & F_BND8) != 0;
+  constexpr int P = 32 / G;
+  const DevScoring& sc = c.sc;
+  const int32_t m = c.m, n = c.n, xs = sc.xclip_suffix;
+  // column 0 (mod.rs:622-671 at i == m).  Its tracker over rows 1..m-1: col0_S never increases with i, so the first
+  // maximum is row 1 (as finish_matrix_coop)
+  int32_t T = MIN_SCORE, Lx0 = 0;
+  if (col0_S(sc, 1) + xs > MIN_SCORE) {
+    T = col0_S(sc, 1) + xs;
+    Lx0 = m - 1;
+  }
+  int32_t Im = col0_I(sc, m);
+  RowM rm{T, MIN_SCORE, TB_XCLIP_SUFFIX, MIN_SCORE, 0};
+  if (Im > rm.Sm) {
+    rm.Sm = Im;
+    rm.sb = TB_INS;
+  }
+  if (sc.xclip_prefix > rm.Sm) {
+    rm.Sm = sc.xclip_prefix;
+    rm.sb = TB_XCLIP_PREFIX;
+  }
+  if (rm.Sm + sc.yclip_suffix > rm.Snm) {
+    rm.Snm = rm.Sm + sc.yclip_suffix;
+    rm.Lym = n;
+  }
+  uint32_t cell = cell_make(col0_ibits(sc, m), TB_START, rm.sb);
+  c.rowm[0 * 32 + c.pi] = (uint16_t)cell;
+  const int32_t p = (int32_t)((c.xs[((m - 1) >> 2) * P + c.g] >> (8 * ((m - 1) & 3))) & 0xffu);  // x[m-1]
+  const uint32_t prow = LUT ? c.lut_base + (uint32_t)(p * sc.alpha * 4) : 0u;
+  const int32_t yclip_score = sc.yclip_prefix + sc.gap_open + sc.gap_extend * (m - 1);
+  int32_t sdiag = col0_S(sc, m - 1), Ti = m;
+  const int2* bnd8 = reinterpret_cast<const int2*>(c.bnd);
+  constexpr int UB = 4;  // four columns' records and y symbols in flight, then the recurrence over them
+  for (int32_t j0 = 1; j0 <= n; j0 += UB) {
+    int4 braw[UB];
+    int32_t qv[UB];
+#pragma unroll
+    for (int u = 0; u < UB; ++u) {
+      const int32_t j = j0 + u;
+      braw[u] = make_int4(0, 0, 0, 0);
+      qv[u] = 0;
+      if (j <= n) {
+        if (B8) {
+          const int2 r8 = bnd8[bnd_index(G, j, c.pi, c.maxn)];
+          braw[u] = make_int4(r8.x, r8.y, 0, 0);
+        } else {
+          braw[u] = c.bnd[bnd_index(G, j, c.pi, c.maxn)];
+        }
+        qv[u] = (int32_t)((c.ys[((j - 1) >> 2) * P + c.g] >> (8 * ((j - 1) & 3))) & 0xffu);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < UB; ++u) {
+      const int32_t j = j0 + u;
+      if (j > n) break;
+      const Boundary b = decode_boundary(braw[u], PK, B8, xs, m);
+      const int32_t q = qv[u];
+      // the score of (x[m-1], y[j-1]): the scaled LUT entry 4*score + 3 - (4*gap_open + 1), or MatchParams
+      const int32_t sub = LUT ? (lut_at(c.lut, prow + (uint32_t)(q * 4)) + 4 * sc.gap_open - 2) >> 2
+                              : (p == q ? sc.match_score : sc.mismatch_score);
+      cell = rowm_cell(sc, n, j, sub, p == q, sdiag, b.S, b.I, b.Tv, yclip_score, rm, Im);
+      if (j == n) {
+        Ti = b.Ti;
+        if (cell_i(cell) == LAZY) cell = cell_set_i(cell, cn.sp);  // the PRE-fix-up s_bits of (m-1, n)
+      }
+      c.rowm[j * 32 + c.pi] = (uint16_t)cell;
+      sdiag = b.S;
+    }
+  }
+  fin_end_state(c, cn, rm, Im, cell, Lx0, m - Ti);
+}
+
 // One strip (rows s*G*R+1 .. (s+1)*G*R) of one lane's pair.
 template <int G, int R, int FLAGS, bool MASKED, int CAPQ>
-B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
+B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s, ColN& cn) {
   constexpr bool TR = (FLAGS & F_TRACK_ROWS) != 0;
   constexpr bool TC = (FLAGS & F_TRACK_COLS) != 0;
   constexpr bool LUT = (FLAGS & F_LUT) != 0;
@@ -344,7 +546,9 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
   constexpr bool B8 = (FLAGS & F_BND8) != 0;           // 8-byte boundary record (with F_PACKTRK only)
   constexpr bool NOTB = (FLAGS & F_NOTB) != 0;         // score-only: no traceback words (c.tb may be null)
   constexpr bool YS = (FLAGS & F_YSTREAM) != 0;        // y read from the arena (warp-per-pair shape only)
+  constexpr bool FIN = (FLAGS & F_FINISH) != 0;
   static_assert(!YS || G == 32, "F_YSTREAM is a warp-per-pair form");
+  static_assert(!FIN || (G == 1 && !PR), "F_FINISH is a thread-per-pair form, without F_PACKREL");
   static_assert(!B8 || ((FLAGS & F_PACKTRK) != 0 && !PR), "F_BND8 needs the packed column tracker with absolute rows");
   constexpr int P = 32 / G;
   constexpr int TBW = tbw_of(R);
@@ -453,7 +657,6 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
   }
   uint4* tbs = NOTB ? nullptr : c.tb + (size_t)s * c.K * TBW * 32;
   const int32_t nsteps = c.K * 8;
-
   if (PR && TR) {
 #pragma unroll
     for (int r = 0; r < R; ++r) {
@@ -527,12 +730,14 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
       }
       int32_t sup = in_s, iup = in_i, Tv = in_tv, Ti = in_ti;
       if (j == n) {
+        if (FIN && s == 0 && rv >= 1) fin_column_n_begin(c, cn);
         column_step<G, R, FLAGS, MASKED, true, CAPQ>(c, j, t, q, rowbase, rv, Sp, Dp, SnR, LyR, tbacc, xc,
-                                               sup_prev, sup, iup, Tv, Ti, cap_s, cap_i);
+                                               sup_prev, sup, iup, Tv, Ti, cap_s, cap_i, cn);
       } else {
         column_step<G, R, FLAGS, MASKED, false, CAPQ>(c, j, t, q, rowbase, rv, Sp, Dp, SnR, LyR, tbacc, xc,
-                                                sup_prev, sup, iup, Tv, Ti, cap_s, cap_i);
+                                                sup_prev, sup, iup, Tv, Ti, cap_s, cap_i, cn);
       }
+
       sup_prev = in_s;
       if (writer) {
         if (B8) {  // one PRMT and one 64-bit store
@@ -614,7 +819,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s) {
         sn = (SnR[r] <= NEG4 / 2) ? MIN_SCORE : (SnR[r] >> 2);
         ly = LyR[r];
       }
-      c.rows[rows_at<G>(ROWS_SN, c.rows_pad, slot)] = sn;
+      if (!FIN) c.rows[rows_at<G>(ROWS_SN, c.rows_pad, slot)] = sn;  // F_FINISH: fix-up 1 used it at column n
       c.rows[rows_at<G>(ROWS_LY, c.rows_pad, slot)] = ly;
     }
   }
@@ -625,6 +830,7 @@ B2A_HD void fill_lane(const LaneCtx<G>& c) {
   // warp-per-pair: the block's traceback has room for its real pairs only (b2a_plan.h), so a task of a padding pair
   // (m = 0) stores nothing.  A real pair with m = 0 has no fill rows either: K2 reads none of its scratch.
   if (G == 32 && c.m == 0) return;
+  ColN cn;  // F_FINISH: column n, carried down the strips in registers (set in strip 0's last column)
   const int32_t s_lo = c.only_strip >= 0 ? c.only_strip : 0;
   const int32_t s_hi = c.only_strip >= 0 ? c.only_strip + 1 : c.nstrips;
   for (int32_t s = s_lo; s < s_hi; ++s) {
@@ -633,23 +839,25 @@ B2A_HD void fill_lane(const LaneCtx<G>& c) {
     // last, partly filled task have m = 0 and simply never become active)
     const bool full = c.uniform && ((s + 1) * (G * R) <= c.maxm - 1);
     if (full) {
-      run_strip<G, R, FLAGS, false, -1>(c, s);
+      run_strip<G, R, FLAGS, false, -1>(c, s, cn);
     } else if (cap_dispatch_of(G) && c.uniform) {
       // uniform block: the one partial lane of the strip (if any) has the same valid-row count for every pair
       const int32_t left = c.maxm - 1 - s * (G * R);  // valid rows from the strip's first row on
       const int32_t part = (left > 0 && left < G * R) ? left % R : 0;
       switch (part ? (part - 1) >> 2 : R / 4) {
-        case 0: run_strip<G, R, FLAGS, true, 0>(c, s); break;
-        case 1: run_strip<G, R, FLAGS, true, (1 <= R / 4 ? 1 : -1)>(c, s); break;
-        case 2: run_strip<G, R, FLAGS, true, (2 <= R / 4 ? 2 : -1)>(c, s); break;
-        case 3: run_strip<G, R, FLAGS, true, (3 <= R / 4 ? 3 : -1)>(c, s); break;
-        case 4: run_strip<G, R, FLAGS, true, (4 <= R / 4 ? 4 : -1)>(c, s); break;
-        case 5: run_strip<G, R, FLAGS, true, (5 <= R / 4 ? 5 : -1)>(c, s); break;
-        default: run_strip<G, R, FLAGS, true, -1>(c, s); break;
+        case 0: run_strip<G, R, FLAGS, true, 0>(c, s, cn); break;
+        case 1: run_strip<G, R, FLAGS, true, (1 <= R / 4 ? 1 : -1)>(c, s, cn); break;
+        case 2: run_strip<G, R, FLAGS, true, (2 <= R / 4 ? 2 : -1)>(c, s, cn); break;
+        case 3: run_strip<G, R, FLAGS, true, (3 <= R / 4 ? 3 : -1)>(c, s, cn); break;
+        case 4: run_strip<G, R, FLAGS, true, (4 <= R / 4 ? 4 : -1)>(c, s, cn); break;
+        case 5: run_strip<G, R, FLAGS, true, (5 <= R / 4 ? 5 : -1)>(c, s, cn); break;
+        default: run_strip<G, R, FLAGS, true, -1>(c, s, cn); break;
       }
     } else {
-      run_strip<G, R, FLAGS, true, -1>(c, s);
+      run_strip<G, R, FLAGS, true, -1>(c, s, cn);
     }
+    // F_FINISH: row m right after the strip that holds row m-1 (a full strip too, when m-1 is a multiple of G*R)
+    if ((FLAGS & F_FINISH) && c.m >= 2 && c.n >= 1 && (c.m - 2) / (G * R) == s) fin_row_m<G, FLAGS>(c, cn);
   }
 }
 
@@ -785,6 +993,10 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
     c.uniform = blk.uniform != 0;
     c.bnd = reinterpret_cast<int4*>(prm.bnd + blk.bnd_off);
     c.rows = reinterpret_cast<int32_t*>(prm.rows + blk.rows_off);
+    if (FLAGS & F_FINISH) {
+      c.rowm = reinterpret_cast<uint16_t*>(prm.rowm + blk.rowm_off);
+      c.fin = prm.fin + (size_t)b * FIN_FIELDS * 32;
+    }
     c.tb = (FLAGS & F_NOTB) ? nullptr
                             : reinterpret_cast<uint4*>(prm.tb + blk.tb_off) + (size_t)sub * blk.nstrips * blk.K * TBW * 32;
     while (!mbar_try_wait(bar, parity)) {

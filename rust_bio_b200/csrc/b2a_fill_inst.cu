@@ -63,6 +63,12 @@ cudaError_t B2A_CAT(B2A_LAUNCH_NAME, B2A_G, B2A_R)(int flags, const FillParams& 
 #define B2A_CASE(F)                                                                    \
   case (NOTB | (F)): return go<(NOTB | (F))>(prm, ntasks, num_sms, stream, grid_out, dry); \
   case (NOTB | F_YSTREAM | (F)): return go<(NOTB | F_YSTREAM | (F))>(prm, ntasks, num_sms, stream, grid_out, dry);
+#elif B2A_G == 1
+  // the thread-per-pair shape finishes each pair's matrix in the fill (F_FINISH) wherever its row trackers are final
+  // at column n, i.e. without F_PACKREL: those cases exist only in the finishing form
+#define B2A_FIN(F) (((F) & F_PACKREL) ? (F) : ((F) | F_FINISH))
+#define B2A_CASE(F) \
+  case (NOTB | B2A_FIN(F)): return go<(NOTB | B2A_FIN(F))>(prm, ntasks, num_sms, stream, grid_out, dry);
 #else
 #define B2A_CASE(F) \
   case (NOTB | (F)): return go<(NOTB | (F))>(prm, ntasks, num_sms, stream, grid_out, dry);

@@ -27,6 +27,7 @@ struct Plan {
   uint64_t seq_bytes = 0, ops_bytes = 0;
   uint64_t max_bnd = 0, max_rows = 0, max_rowm = 0, max_tb = 0;  // per-wave maxima
   uint64_t max_strip_tasks = 0;
+  uint64_t max_fin = 0;    // F_FINISH: bytes of the finish region of the wave with the most blocks (else 0)
   uint64_t total_tb = 0;   // traceback bytes the fill stores over the whole batch
   uint64_t cells = 0;
   uint32_t smem_seq_bytes = 0;  // per-warp staging
@@ -37,7 +38,7 @@ inline uint64_t align_up(uint64_t v, uint64_t a) { return (v + a - 1) / a * a; }
 
 // `flags`: the fill's kernel flags (F_BND8 halves the boundary record; F_NOTB, a score-only batch, stores no
 // traceback, and its waves close on the rest of the per-wave scratch -- boundary rows, rows arena, row-m cells --
-// against the same budget).
+// against the same budget; F_FINISH adds the finish region, max_fin, and changes nothing else).
 // Blocks hold 32 pairs (the last one the rest), except in the warp-per-pair shape (G == 32) with a traceback: there a
 // block's traceback is sized by its real pairs, and a block closes early when its next pair would take it past
 // `tb_budget`, so that waves can close between long pairs.  A single pair above the budget still gets a block (and a
@@ -97,6 +98,7 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
   p.seq_bytes = p.ops_bytes = 0;
   p.max_bnd = p.max_rows = p.max_rowm = p.max_tb = 0;
   p.max_strip_tasks = 0;
+  p.max_fin = 0;
   p.total_tb = 0;
   p.smem_seq_bytes = 0;
   p.maxm = p.maxn = 0;
@@ -161,6 +163,8 @@ inline void build_plan(Plan& p, const uint32_t* x_len, const uint32_t* y_len, ui
     p.max_rowm = std::max(p.max_rowm, v.rowm_bytes);
     p.max_tb = std::max(p.max_tb, v.tb_bytes);
     p.max_strip_tasks = std::max(p.max_strip_tasks, v.strip_tasks);
+    if (flags & F_FINISH)  // FIN_FIELDS words per pair of every block of the wave
+      p.max_fin = std::max<uint64_t>(p.max_fin, (uint64_t)(v.block_hi - v.block_lo) * FIN_FIELDS * 32 * 4);
   }
 }
 

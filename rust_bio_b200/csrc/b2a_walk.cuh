@@ -9,7 +9,9 @@
 //   Alignment construction / clip filtering                 910-921, 974, 1006
 // These parts are sequential per pair and O(m+n); they are replayed literally
 // here on top of what K1 left in HBM: the boundary row m-1 (S, I, column
-// tracker), the row trackers, the last column and the 4-bit traceback.
+// tracker), the row trackers, the last column and the 4-bit traceback.  A
+// thread-per-pair fill with F_FINISH has already done row m and the fix-ups
+// (rowm_cell below is shared with it) and left each pair's EndState: K2 loads it.
 #pragma once
 #include "b2a_common.cuh"
 #include "b2a_coop.cuh"
@@ -34,6 +36,7 @@ struct WalkParams {
   int32_t filter_clips;  // semiglobal / local: Alignment::filter_clip_operations
   int32_t packtrk;       // K1 ran with F_PACKTRK (how the column tracker in the boundary row is encoded)
   int32_t bnd8;          // K1 ran with F_BND8 (8-byte boundary records)
+  const int32_t* fin;    // K1 ran with F_FINISH: its finish region (FIN_* in b2a_common.cuh), else null
   uint32_t seq_smem_per_warp;  // warp-per-pair K2: bytes of shared memory per warp for the pair's x and y (0: none)
   // outputs, indexed by the caller's pair index
   int32_t* score;
@@ -59,6 +62,11 @@ B2A_HD T ldg_ro(const T* p) {
 #endif
 }
 
+// s_bits of an interior nibble whose source is not the diagonal (NB_DIAG: Match / Subst by symbol equality)
+B2A_HD uint32_t nib_scode_other(uint32_t nb) {
+  return (nb & 3u) == NB_INS ? (uint32_t)TB_INS : (nb & 3u) == NB_DEL ? (uint32_t)TB_DEL : (uint32_t)TB_XCLIP_PREFIX;
+}
+
 struct PairView {
   DevScoring sc;
   const int32_t* lut;
@@ -78,6 +86,7 @@ struct PairView {
   int32_t maxn;        // block maximum of n
   int64_t bnd_base;    // boundary row of this pair: bnd[bnd_base + j * bnd_stride] (see bnd_index)
   int32_t bnd_stride;
+  const int32_t* fin = nullptr;  // F_FINISH fill: the block's finish region ([field][32]), else null
   const uint8_t* xs8 = nullptr;  // warp-per-pair K2: the pair's staged x / y copied into shared memory (or null)
   const uint8_t* ys8 = nullptr;
   // exact division by R and by G*R without a divide: q = (x * mul) >> 40 with mul = ceil(2^40 / d) is floor(x / d)
@@ -127,13 +136,10 @@ struct PairView {
     return (tb[word] >> (4 * (7 - (t & 7)))) & 15u;
   }
   B2A_HD uint32_t nib_scode(uint32_t nb, int32_t i, int32_t j) const {
-    switch (nb & 3u) {
-      case NB_DIAG: return xsym(i) == ysym(j) ? TB_MATCH : TB_SUBST;
-      case NB_INS: return TB_INS;
-      case NB_DEL: return TB_DEL;
-      default: return TB_XCLIP_PREFIX;
-    }
+    return (nb & 3u) == NB_DIAG ? (xsym(i) == ysym(j) ? TB_MATCH : TB_SUBST) : nib_scode_other(nb);
   }
+  // the fused finish ran in K1 for this pair: K2 only loads its EndState (load_end_state)
+  B2A_HD bool finished() const { return fin != nullptr && m >= 2 && n >= 1; }
 };
 
 // Boundary row m-1 as K1 leaves it (scaled domain, b2a_fill.cuh): x = 4*S, y = 4*I + 2,
@@ -184,6 +190,93 @@ struct EndState {
   int32_t Lx0, LxN;   // Lx[0], Lx[n]
 };
 
+// Row m as it runs along the columns: S, D and s_bits of the last column done, and the row tracker Sn[m], Ly[m].
+struct RowM {
+  int32_t Sm, Dm;  // S(m, j-1), D(m, j-1)
+  uint32_t sb;     // s_bits(m, j-1)
+  int32_t Snm, Lym;
+};
+
+// Cell (m, j), 1 <= j <= n (mod.rs:729-805 at i == m, the running best starting from the column tracker, 641-645),
+// literally.  Inputs: the score of (x[m-1], y[j-1]) and whether the two symbols are equal, S(m-1, j-1), and S, I and
+// the column tracker (value Tv) of (m-1, j).  Returns the u16 cell; its i_bits are LAZY when I came from S(m-1, j)
+// (the walk resolves them from s_bits(m-1, j); at j == n the caller does, from the PRE-fix-up s_bits of (m-1, n)).
+// Advances `st` to column j and returns I(m, j) in `Im`.  Shared by K2 (finish_matrix_seq) and the F_FINISH fill.
+B2A_HD uint32_t rowm_cell(const DevScoring& sc, const int32_t n, const int32_t j, const int32_t sub, const bool same,
+                          const int32_t sdiag, const int32_t sup, const int32_t iup, const int32_t Tv,
+                          const int32_t yclip_score, RowM& st, int32_t& Im) {
+  const int32_t go = sc.gap_open, ge = sc.gap_extend;
+  const int32_t m_score = sdiag + sub;
+  int32_t best_i;
+  uint32_t ib;
+  {
+    const int32_t i_score = iup + ge, s_score = sup + go;
+    if (i_score > s_score) {
+      best_i = i_score;
+      ib = TB_INS;
+    } else {
+      best_i = s_score;
+      ib = LAZY;
+    }
+  }
+  int32_t best_d;
+  uint32_t db;
+  {
+    const int32_t d_score = st.Dm + ge, s_score = st.Sm + go;
+    if (d_score > s_score) {
+      best_d = d_score;
+      db = TB_DEL;
+    } else {
+      best_d = s_score;
+      db = st.sb;  // s_bits of (m, j-1), final for j-1 < n
+    }
+  }
+  int32_t best = Tv;
+  uint32_t sb = TB_XCLIP_SUFFIX;
+  if (m_score > best) {
+    best = m_score;
+    sb = same ? TB_MATCH : TB_SUBST;
+  }
+  if (best_i > best) {
+    best = best_i;
+    sb = TB_INS;
+  }
+  if (best_d > best) {
+    best = best_d;
+    sb = TB_DEL;
+  }
+  const int32_t xcs = xclip_score(sc, j);
+  if (xcs > best) {
+    best = xcs;
+    sb = TB_XCLIP_PREFIX;
+  }
+  if (yclip_score > best) {
+    best = yclip_score;
+    sb = TB_YCLIP_PREFIX;
+  }
+  st.Sm = best;
+  st.Dm = best_d;
+  st.sb = sb;
+  Im = best_i;
+  if (best + sc.yclip_suffix > st.Snm) {
+    st.Snm = best + sc.yclip_suffix;
+    st.Lym = n - j;
+  }
+  return cell_make(ib, db, sb);
+}
+
+// The EndState an F_FINISH fill left for one pair (b2a_fill.cuh): fields [f * 32 + pi] of the block's finish region
+B2A_HD void load_end_state(const PairView& v, EndState& es) {
+  const int32_t* f = v.fin + v.pi;
+  es.SmN = ldg_ro(f + FIN_SMN * 32);
+  es.ImN = ldg_ro(f + FIN_IMN * 32);
+  es.cmN = (uint32_t)ldg_ro(f + FIN_CMN * 32);
+  es.Snm = ldg_ro(f + FIN_SNM * 32);
+  es.Lym = ldg_ro(f + FIN_LYM * 32);
+  es.Lx0 = ldg_ro(f + FIN_LX0 * 32);
+  es.LxN = ldg_ro(f + FIN_LXN * 32);
+}
+
 // Row m (mod.rs:641-645, 729-805 at i == m), the two last-column fix-up passes (809-843): one lane, literally.
 B2A_HD void finish_matrix_seq(const PairView& v, EndState& es) {
   const DevScoring& sc = v.sc;
@@ -223,7 +316,7 @@ B2A_HD void finish_matrix_seq(const PairView& v, EndState& es) {
       Snm = Sm + ys;
       Lym = n;
     }
-    int32_t Dm = MIN_SCORE;
+    RowM st{Sm, MIN_SCORE, sb, Snm, Lym};
     uint32_t cell = cell_make(ib, TB_START, sb);
     v.rowm[0 * 32 + v.pi] = (uint16_t)cell;
     LxN = Lx0;
@@ -264,74 +357,23 @@ B2A_HD void finish_matrix_seq(const PairView& v, EndState& es) {
         Ti = b.Ti;
       }
       const int32_t q = qv[u];
-      const int32_t m_score = sdiag + v.score(p, q);
-      int32_t best_i, best_d;
-      {
-        const int32_t i_score = iup + ge, s_score = sup + go;
-        if (i_score > s_score) {
-          best_i = i_score;
-          ib = TB_INS;
-        } else {
-          best_i = s_score;
-          ib = LAZY;
-        }
-      }
-      uint32_t db;
-      {
-        const int32_t d_score = Dm + ge, s_score = Sm + go;
-        if (d_score > s_score) {
-          best_d = d_score;
-          db = TB_DEL;
-        } else {
-          best_d = s_score;
-          db = sb;  // s_bits of (m, j-1), final for j-1 < n
-        }
-      }
-      int32_t best = Tv;
-      sb = TB_XCLIP_SUFFIX;
-      if (m_score > best) {
-        best = m_score;
-        sb = (p == q) ? TB_MATCH : TB_SUBST;
-      }
-      if (best_i > best) {
-        best = best_i;
-        sb = TB_INS;
-      }
-      if (best_d > best) {
-        best = best_d;
-        sb = TB_DEL;
-      }
-      const int32_t xcs = xclip_score(sc, j);
-      if (xcs > best) {
-        best = xcs;
-        sb = TB_XCLIP_PREFIX;
-      }
-      if (yclip_score > best) {
-        best = yclip_score;
-        sb = TB_YCLIP_PREFIX;
-      }
-      Sm = best;
-      Im = best_i;
-      Dm = best_d;
-      if (Sm + ys > Snm) {
-        Snm = Sm + ys;
-        Lym = n - j;
-      }
+      cell = rowm_cell(sc, n, j, v.score(p, q), p == q, sdiag, sup, iup, Tv, yclip_score, st, Im);
       if (j == n) {
         LxN = m - Ti;
-        if (ib == LAZY) {  // i_bits captured before the fix-ups touch (m-1, n)
-          ib = (m == 1) ? row0_sbits(sc, n, n)
-                        : v.nib_scode((uint32_t)v.row(ROWS_NL, m - 1), m - 1, n);
+        if (cell_i(cell) == LAZY) {  // i_bits captured before the fix-ups touch (m-1, n)
+          cell = cell_set_i(cell, (m == 1) ? row0_sbits(sc, n, n)
+                                           : v.nib_scode((uint32_t)v.row(ROWS_NL, m - 1), m - 1, n));
         }
       }
-      cell = cell_make(ib, db, sb);
       v.rowm[j * 32 + v.pi] = (uint16_t)cell;
       sdiag = sup;
           }
     }
-    SmN = Sm;
+    SmN = st.Sm;
     ImN = Im;
     cmN = cell;
+    Snm = st.Snm;
+    Lym = st.Lym;
   }
 
   // ------------------------------- column n: materialise the cells K1 left as nibbles and run fix-up 1
@@ -682,7 +724,8 @@ B2A_HD void walk_finish(const EndState& es, const WalkState& w, WalkOut& out) {
 template <bool SCORES = false>
 B2A_HD void walk_pair(const PairView& v, const bool filter_clips, uint8_t* ops_end, WalkOut& out) {
   EndState es;
-  finish_matrix_seq(v, es);
+  if (v.finished()) load_end_state(v, es);
+  else finish_matrix_seq(v, es);
   WalkState w;
   walk_begin(v, es, ops_end, w);
   walk_run<SCORES>(v, es, filter_clips, w, 0x7fffffff);
@@ -745,6 +788,10 @@ B2A_HD void finish_matrix_coop(const int lane, const PairView& v, EndState& es) 
   using C = Coop<W>;
   const DevScoring& sc = v.sc;
   const int32_t m = v.m, n = v.n;
+  if (v.finished()) {  // the F_FINISH fill did row m and the fix-ups
+    load_end_state(v, es);
+    return;
+  }
   if (m < 2 || n < 1) {  // degenerate shapes: closed forms only, nothing to share out
     if (lane == 0) finish_matrix_seq(v, es);
     C::sync();
@@ -1147,7 +1194,7 @@ __device__ __forceinline__ void walk_store(const WalkParams& prm, const Block& b
 
 // K2 for one pair (lane) of a block
 template <bool SCORES>
-__device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& blk, const int lane) {
+__device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& blk, const uint32_t b, const int lane) {
   if ((uint32_t)lane >= blk.npairs) return;
   const uint32_t sp = blk.first + lane;
   const int32_t P = 32 / prm.G;
@@ -1165,6 +1212,7 @@ __device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& bl
   v.g = lane % P;
   v.packtrk = prm.packtrk;
   v.bnd8 = prm.bnd8;
+  v.fin = prm.fin ? prm.fin + (size_t)b * FIN_FIELDS * 32 : nullptr;
   v.maxn = (int32_t)blk.maxn;
   v.bnd_base = bnd_index(prm.G, 0, lane, v.maxn);
   v.bnd_stride = (int32_t)(bnd_index(prm.G, 1, lane, v.maxn) - v.bnd_base);
@@ -1185,7 +1233,7 @@ __device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& bl
 
 // K2, one warp per pair
 template <bool SCORES>
-__device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& blk, const int pi, const int lane,
+__device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& blk, const uint32_t b, const int pi, const int lane,
                                           uint8_t* seq_smem) {
   const uint32_t sp = blk.first + pi;
   const int32_t P = 32 / prm.G;
@@ -1203,6 +1251,7 @@ __device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& bl
   v.g = pi % P;
   v.packtrk = prm.packtrk;
   v.bnd8 = prm.bnd8;
+  v.fin = prm.fin ? prm.fin + (size_t)b * FIN_FIELDS * 32 : nullptr;
   v.maxn = (int32_t)blk.maxn;
   v.bnd_base = bnd_index(prm.G, 0, pi, v.maxn);
   v.bnd_stride = (int32_t)(bnd_index(prm.G, 1, pi, v.maxn) - v.bnd_base);
@@ -1245,7 +1294,7 @@ __global__ void __launch_bounds__(1024, 1) walk_warp_kernel(const WalkParams prm
   const Block blk = prm.blocks[b];
   if (pi >= blk.npairs) return;
   uint8_t* mine = prm.seq_smem_per_warp ? walk_smem + (size_t)(threadIdx.x >> 5) * prm.seq_smem_per_warp : nullptr;
-  walk_warp<SCORES>(prm, blk, (int)pi, lane, mine);
+  walk_warp<SCORES>(prm, blk, b, (int)pi, lane, mine);
 }
 
 template <bool SCORES>
@@ -1254,7 +1303,7 @@ __global__ void __launch_bounds__(128, 8) walk_kernel(const WalkParams prm) {
   const int lane = threadIdx.x & 31;
   if (gw >= prm.nblocks) return;
   const Block blk = prm.blocks[gw];
-  walk_lane<SCORES>(prm, blk, lane);
+  walk_lane<SCORES>(prm, blk, gw, lane);
 }
 #endif
 
