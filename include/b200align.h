@@ -143,7 +143,8 @@ typedef struct b2a_stats {
   uint64_t cells;          /* sum of DP cells (m*n, or Band::num_cells for banded) */
   uint64_t h2d_bytes;
   uint64_t d2h_bytes;
-  uint64_t traceback_bytes; /* traceback bit-vector bytes the fill kernel stores */
+  uint64_t traceback_bytes; /* traceback bit-vector bytes the fill kernel stores (a recomputed pair: what its refills
+                                store, window by window) */
   float pack_ms;           /* K0 */
   float fill_ms;           /* K1 (or K3) */
   float walk_ms;           /* K2 epilogue + traceback walk (+ ops compaction) */
@@ -167,8 +168,19 @@ int32_t b2a_engine_set_stream(b2a_engine* e, void* cuda_stream);
 /* Upper bound (bytes) on device scratch for traceback bit-vectors; larger
  * batches are processed in waves. 0 = default (60% of free HBM).  With the warp-per-pair shape a block holds fewer
  * than 32 pairs when that keeps it within the budget, so waves can close between long pairs; a single pair whose
- * traceback alone is above the budget is B2A_E_UNSUPPORTED before anything is allocated. */
+ * traceback alone is above the budget is B2A_E_UNSUPPORTED before anything is allocated, unless the traceback
+ * recompute knob below is on. */
 int32_t b2a_engine_set_traceback_budget(b2a_engine* e, uint64_t bytes);
+/* on = 1: a warp-per-pair pair whose traceback alone is above the budget is aligned anyway, by recomputation: one
+ * extra score-only fill checkpoints the strip boundary every W = floor(budget / strip bytes) strips, and the traceback
+ * is refilled one window of W strips at a time as the walk reaches it (windows the walk jumps over are never filled).
+ * Results are bit-identical to a budget that holds the pair.  Such a batch costs at least one more fill and a host
+ * round trip per window.  A budget below one strip's traceback of the pair (K * TBW * 512 bytes) is still
+ * B2A_E_UNSUPPORTED.  on = 0 (the default) keeps the refusal.  The chunk pipeline's engines inherit the setting. */
+int32_t b2a_engine_set_traceback_recompute(b2a_engine* e, int32_t on);
+/* Of the last b2a_align_batch / b2a_batch_stage + run: the pairs whose traceback was recomputed, their windows, and the
+ * windows actually refilled (a measurement aid; any pointer may be NULL). */
+int32_t b2a_engine_last_recompute(const b2a_engine* e, uint64_t* pairs, uint64_t* windows, uint64_t* windows_filled);
 /* Force the fill-kernel shape (lanes per pair G in {1,2,4,8,32}, rows per
  * lane R in {8,16,20}: the built pairs are 1x8 1x16 1x20 2x16 2x20 4x16 8x16 8x20 32x8 32x16); 0,0 = automatic.
  * The shapes with several pairs per warp stage whole sequences in shared memory: forced, a batch they cannot stage

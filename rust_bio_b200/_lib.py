@@ -24,6 +24,7 @@ ABI_SYMBOLS = [
     "b2a_engine_create", "b2a_engine_destroy", "b2a_last_error", "b2a_version",
     "b2a_engine_set_stream", "b2a_engine_set_traceback_budget", "b2a_engine_set_tuning",
     "b2a_engine_set_pipeline", "b2a_engine_set_walk", "b2a_engine_last_alphabet",
+    "b2a_engine_set_traceback_recompute", "b2a_engine_last_recompute",
     "b2a_align_batch", "b2a_align_batch_banded", "b2a_align_batch_banded_hinted", "b2a_banded_band_ranges", "b2a_banded_strip_pairs", "b2a_batch_stage", "b2a_batch_run",
     "b2a_batch_stage_scores", "b2a_align_batch_scores", "b2a_align_batch_banded_scores",
     "b2a_batch_fetch", "b2a_batch_records", "b2a_batch_records_into", "b2a_record_stride",
@@ -105,6 +106,9 @@ def load():
     L.b2a_engine_destroy.argtypes = [C.c_void_p]
     L.b2a_engine_set_stream.argtypes = [C.c_void_p, C.c_void_p]
     L.b2a_engine_set_traceback_budget.argtypes = [C.c_void_p, C.c_uint64]
+    L.b2a_engine_set_traceback_recompute.argtypes = [C.c_void_p, C.c_int32]
+    L.b2a_engine_last_recompute.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
+                                            C.POINTER(C.c_uint64)]
     L.b2a_engine_set_tuning.argtypes = [C.c_void_p, C.c_int32, C.c_int32]
     L.b2a_engine_set_pipeline.argtypes = [C.c_void_p, C.c_int32]
     L.b2a_engine_set_walk.argtypes = [C.c_void_p, C.c_int32]

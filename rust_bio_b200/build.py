@@ -21,6 +21,8 @@ SO = os.path.join(CSRC, "libb200align%s.so" % (("_" + VARIANT) if VARIANT else "
 SHAPES = [(1, 16), (1, 8), (1, 20), (2, 16), (2, 20), (4, 16), (8, 16), (8, 20), (32, 8), (32, 16)]
 # the shapes the engine's automatic choice picks also get the score-only (F_NOTB) fill, in translation units of their own
 NOTB_SHAPES = [(1, 16), (8, 16), (8, 20), (32, 8), (32, 16)]
+# the warp-per-pair shapes also get the recomputed-traceback fills (a pair above the traceback budget), in their own units
+RECOMPUTE_SHAPES = [(32, 8), (32, 16)]
 # minimum resident CTAs per SM asked of ptxas per shape (__launch_bounds__): measured choice, see DESIGN.md
 MIN_BLOCKS = {(1, 16): int(os.environ.get("B2A_MINB_1_16", "3")), (8, 16): int(os.environ.get("B2A_MINB_8_16", "3")),
               (8, 20): int(os.environ.get("B2A_MINB_8_20", "1"))}  # 8x20 at 3 CTAs/SM (168 registers) was slower
@@ -61,13 +63,14 @@ def build(force: bool = False, verbose: bool = False) -> str:
     jobs = []
     objs = []
     src = os.path.join(CSRC, "b2a_fill_inst.cu")
-    for notb, shapes in ((False, SHAPES), (True, NOTB_SHAPES)):
+    for kind, shapes in (("", SHAPES), ("notb_", NOTB_SHAPES), ("recompute_", RECOMPUTE_SHAPES)):
         for g, r in shapes:
-            o = os.path.join(OBJ, f"fill_{'notb_' if notb else ''}{g}_{r}.o")
+            o = os.path.join(OBJ, f"fill_{kind}{g}_{r}.o")
             objs.append(o)
             if force or _stale(o, hdrs + [src]):
+                defs = {"": [], "notb_": ["-DB2A_NOTB"], "recompute_": ["-DB2A_RECOMPUTE"]}[kind]
                 jobs.append([NVCC, *FLAGS, f"-DB2A_G={g}", f"-DB2A_R={r}", f"-DB2A_MINB={MIN_BLOCKS.get((g, r), 1)}",
-                             *(["-DB2A_NOTB"] if notb else []), "-c", src, "-o", o])
+                             *defs, "-c", src, "-o", o])
     eo = os.path.join(OBJ, "engine.o")
     objs.append(eo)
     esrc = os.path.join(CSRC, "b2a_engine.cu")

@@ -94,6 +94,12 @@ enum : int {
   F_FINISH = 2048,   // thread-per-pair fill (G == 1) without F_PACKREL: the lane also computes row m, the literal cells of
                      // column n and both last-column fix-ups, and leaves each pair's EndState in the finish region
                      // (FIN_* below) instead of S, I and the row trackers of column n in the rows arena (DESIGN.md §2)
+  // Recomputed traceback (warp-per-pair shape, a pair whose traceback is above the budget; DESIGN.md §2):
+  F_CKPT = 4096,     // with F_NOTB: the writer of a strip that ends a window of W strips also stores its boundary record
+                     // into that window's checkpoint row
+  F_REFILL = 8192,   // fills only the strips [lo, hi) of one window (no trackers): strip lo reads its top boundary from a
+                     // scratch row seeded from a checkpoint, every strip hands on through that row, the traceback goes at
+                     // window-relative strip offsets, and nothing is written to the rows arena
 };
 // The finish region of an F_FINISH fill: FIN_FIELDS int32 per pair, [field][32] per block, blocks in wave order: the
 // EndState K2 reads (b2a_walk.cuh).

@@ -65,8 +65,8 @@ const FillLaunch kFillShapes[] = {
     {4, 16, launch_fill_4_16, nullptr},
     {8, 16, launch_fill_8_16, launch_fill_notb_8_16},
     {8, 20, launch_fill_8_20, launch_fill_notb_8_20},
-    {32, 8, launch_fill_32_8, launch_fill_notb_32_8},
-    {32, 16, launch_fill_32_16, launch_fill_notb_32_16},
+    {32, 8, launch_fill_32_8, launch_fill_notb_32_8, launch_fill_recompute_32_8},
+    {32, 16, launch_fill_32_16, launch_fill_notb_32_16, launch_fill_recompute_32_16},
 };
 
 const FillLaunch* find_shape(int G, int R) {
@@ -125,6 +125,14 @@ struct b2a_engine {
   std::vector<uint64_t> eff_xoff, eff_yoff;
   bool last_walk_warp = false;
   uint64_t tb_budget = 0;
+  bool tb_recompute = false;  // b2a_engine_set_traceback_recompute: a pair above the budget gets its traceback recomputed
+  // a wave of the staged batch whose one pair's traceback is recomputed: W strips per window, ceil(nstrips / W) windows
+  struct RecomputeWave {
+    uint32_t wave, win, windows;
+  };
+  std::vector<RecomputeWave> rc_waves;
+  uint64_t rc_pairs = 0, rc_windows = 0, rc_filled = 0;  // of the last call (b2a_engine_last_recompute)
+  uint64_t rc_tb_stored = 0;  // traceback bytes the refills of the last run stored (plan.total_tb leaves those pairs out)
 
   // batch state
   bool staged = false, ran = false;
@@ -143,7 +151,7 @@ struct b2a_engine {
       d_rowm, d_fin, d_tb, d_opsscratch, d_lut, d_codemap, d_ctl, d_score, d_xs, d_xe, d_ys, d_ye, d_nops,
       d_opssrc, d_clip, d_status, d_nops64, d_opsoff, d_opsdense, d_scan, d_records, d_prog, d_bcells, d_bstatus,
       d_bopsend, d_bslab, d_branges, d_broff, d_bfill, d_bfoff, d_hmoff, d_hmxy, d_hpoff, d_hpidx, d_raw, d_gnops,
-      d_gnops64, d_goff, d_bcols, d_bstrip, d_bsoff, d_belig;
+      d_gnops64, d_goff, d_bcols, d_bstrip, d_bsoff, d_belig, d_ckpt, d_rcbnd, d_rcstate;
   uint32_t* h_nops = nullptr;  // pinned staging of b2a_gathered_fetch
   uint64_t h_nops_cap = 0;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -333,7 +341,8 @@ int32_t b2a_engine_destroy(b2a_engine* e) {
                     &e->d_nops64, &e->d_opsoff, &e->d_opsdense, &e->d_scan, &e->d_records, &e->d_prog, &e->d_bcells,
                     &e->d_bstatus, &e->d_bopsend, &e->d_bslab, &e->d_branges, &e->d_broff, &e->d_bfill, &e->d_hmoff, &e->d_hmxy,
                     &e->d_hpoff, &e->d_hpidx, &e->d_raw, &e->d_gnops, &e->d_gnops64, &e->d_goff,
-                    &e->d_bfoff, &e->d_bcols, &e->d_bstrip, &e->d_bsoff, &e->d_belig};
+                    &e->d_bfoff, &e->d_bcols, &e->d_bstrip, &e->d_bsoff, &e->d_belig, &e->d_ckpt, &e->d_rcbnd,
+                    &e->d_rcstate};
   for (DevBuf* b : bufs) b->release();
   for (auto& v : e->ev)
     if (v) cudaEventDestroy(v);
@@ -352,6 +361,21 @@ int32_t b2a_engine_set_stream(b2a_engine* e, void* cuda_stream) {
 int32_t b2a_engine_set_traceback_budget(b2a_engine* e, uint64_t bytes) {
   if (!e) return B2A_E_INVALID;
   e->tb_budget = bytes;
+  return B2A_OK;
+}
+
+int32_t b2a_engine_set_traceback_recompute(b2a_engine* e, int32_t on) {
+  if (!e) return B2A_E_INVALID;
+  if (on != 0 && on != 1) return e->fail(B2A_E_INVALID, "traceback recompute must be 0 (off) or 1 (on)");
+  e->tb_recompute = on != 0;
+  return B2A_OK;
+}
+
+int32_t b2a_engine_last_recompute(const b2a_engine* e, uint64_t* pairs, uint64_t* windows, uint64_t* windows_filled) {
+  if (!e) return B2A_E_INVALID;
+  if (pairs) *pairs = e->rc_pairs;
+  if (windows) *windows = e->rc_windows;
+  if (windows_filled) *windows_filled = e->rc_filled;
   return B2A_OK;
 }
 
@@ -396,6 +420,8 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
   if (!e || !s || !pairs) return B2A_E_INVALID;
   e->staged = e->ran = false;
   e->score_only = false;
+  e->rc_waves.clear();
+  e->rc_pairs = e->rc_windows = e->rc_filled = 0;
   if (mode < 0 || mode > 3) return e->fail(B2A_E_INVALID, "mode must be B2A_MODE_*");
   int rc = validate_scoring(e, s);
   if (rc) return rc;
@@ -593,6 +619,43 @@ static int32_t compact_ops(b2a_engine* e, uint64_t scratch_bytes, cudaStream_t s
   return B2A_OK;
 }
 
+// traceback bytes of one strip of a warp-per-pair block's pair
+static uint64_t strip_tb(const Plan& pl, const Block& k) { return (uint64_t)k.K * tbw_of(pl.R) * 512; }
+
+// A full batch whose warp-per-pair plan holds a pair above the traceback budget, with the recompute knob on
+// (DESIGN.md §2 "recomputed traceback"): such a pair has a block and a wave of its own, and its traceback is refilled
+// one window of W = floor(budget / strip bytes) strips at a time.  The batch switches to the record those fills share:
+// 16-byte boundary records with relative packed keys (F_PACKREL) in place of F_PACKTRK / F_BND8, and y read from the
+// arena (F_YSTREAM).  The other pairs give the same results with these flags.
+static int32_t plan_recompute(b2a_engine* e, const b2a_pairs* pairs, uint64_t budget, int64_t score_bound) {
+  if (!e->shape->launch_recompute) return e->fail(B2A_E_UNSUPPORTED, "no recomputing fill for this shape");
+  const bool trackers = (e->flags & (F_TRACK_ROWS | F_TRACK_COLS)) != 0;
+  e->flags &= ~(F_PACKTRK | F_BND8);
+  if (trackers && score_bound < (1ll << 18) && !e->no_packrel) e->flags |= F_PACKREL;
+  e->flags |= F_YSTREAM;
+  Plan& pl = e->plan;
+  build_plan(pl, pairs->x_len, pairs->y_len, e->n_pairs, pl.G, pl.R, budget, e->flags);
+  pl.smem_seq_bytes = (uint32_t)(pl.G * pl.R);  // F_YSTREAM stages one strip of x
+  for (size_t wv = 0; wv < pl.waves.size(); ++wv) {
+    const Wave& w = pl.waves[wv];
+    if (w.tb_bytes <= budget) continue;
+    const Block& k = pl.blocks[w.block_lo];
+    if (w.block_hi - w.block_lo != 1 || k.npairs != 1)  // (b2a_plan.h gives such a pair a block and a wave alone)
+      return e->fail(B2A_E_UNSUPPORTED, "a wave above the traceback budget holds more than one pair");
+    const uint64_t stb = strip_tb(pl, k);
+    if (budget < stb)
+      return e->fail(B2A_E_UNSUPPORTED, "a recomputed traceback is refilled one window of strips at a time, and one "
+                                        "strip of this pair's traceback needs " + std::to_string(stb) +
+                                        " bytes, above the traceback budget of " + std::to_string(budget) + " bytes");
+    const uint32_t win = (uint32_t)std::min<uint64_t>(budget / stb, k.nstrips);
+    e->rc_waves.push_back({(uint32_t)wv, win, (k.nstrips + win - 1) / win});
+    pl.total_tb -= (uint64_t)k.nstrips * stb;  // never stored whole: the refills count what they store
+    ++e->rc_pairs;
+    e->rc_windows += e->rc_waves.back().windows;
+  }
+  return B2A_OK;
+}
+
 extern "C" {
 
 // score_only: the batch of b2a_batch_stage_scores -- the fill's F_NOTB twin and a plan without traceback bytes
@@ -652,7 +715,11 @@ static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* 
                                       "8x20, 32x8, 32x16); the forced shape has no score-only fill kernel");
   const Plan& pl = e->plan;
   // the warp-per-pair plan gives a pair whose traceback alone is above the budget a block of its own (b2a_plan.h)
-  if (!score_only && pl.G == 32 && pl.max_tb > budget)
+  if (!score_only && pl.G == 32 && pl.max_tb > budget && e->tb_recompute) {
+    rc = plan_recompute(e, pairs, budget, score_bound);
+    if (rc) return rc;
+  }
+  if (!score_only && pl.G == 32 && pl.max_tb > budget && e->rc_waves.empty())
     return e->fail(B2A_E_UNSUPPORTED, "a pair's traceback needs " + std::to_string(pl.max_tb) +
                                           " bytes, above the traceback budget of " + std::to_string(budget) +
                                           " bytes; the score-only calls (b2a_align_batch_scores, b2a_batch_stage_scores) "
@@ -672,7 +739,28 @@ static int32_t batch_stage_impl(b2a_engine* e, int32_t mode, const b2a_scoring* 
   CK(e->d_rows.reserve(pl.max_rows + 16));
   CK(e->d_rowm.reserve(pl.max_rowm + 16));
   CK(e->d_fin.reserve(pl.max_fin + 16));
-  CK(e->d_tb.reserve(pl.max_tb + 16));
+  {
+    // a recomputed wave holds one window of its pair's traceback, and the window checkpoints
+    uint64_t tb_bytes = 0, ckpt_bytes = 0, row_bytes = 0;
+    size_t next = 0;
+    for (size_t wv = 0; wv < pl.waves.size(); ++wv) {
+      if (next < e->rc_waves.size() && e->rc_waves[next].wave == wv) {
+        const b2a_engine::RecomputeWave& rw = e->rc_waves[next++];
+        const Block& k = pl.blocks[pl.waves[wv].block_lo];
+        tb_bytes = std::max<uint64_t>(tb_bytes, (uint64_t)rw.win * strip_tb(pl, k));
+        ckpt_bytes = std::max<uint64_t>(ckpt_bytes, (uint64_t)(rw.windows - 1) * (k.maxn + 1) * 16);
+        row_bytes = std::max<uint64_t>(row_bytes, (uint64_t)(k.maxn + 1) * 16);
+      } else {
+        tb_bytes = std::max<uint64_t>(tb_bytes, pl.waves[wv].tb_bytes);
+      }
+    }
+    CK(e->d_tb.reserve(tb_bytes + 16));
+    if (!e->rc_waves.empty()) {
+      CK(e->d_ckpt.reserve(ckpt_bytes + 16));
+      CK(e->d_rcbnd.reserve(row_bytes + 16));
+      CK(e->d_rcstate.reserve(1024));
+    }
+  }
   CK(e->d_prog.reserve(pl.max_strip_tasks * 4 + 16));
   CK(e->d_opsscratch.reserve(pl.ops_bytes + 16));
   CK(e->d_lut.reserve(e->lut_host.size() * 4 + 16));
@@ -739,6 +827,78 @@ int32_t b2a_batch_stage_scores(b2a_engine* e, int32_t mode, const b2a_scoring* s
   return batch_stage_impl(e, mode, s, pairs, true);
 }
 
+// One recomputed wave (plan_recompute): pass 1 fills the pair without a traceback and checkpoints the boundary row at
+// every window's end (F_NOTB | F_CKPT); then K2 runs in segments (walk_window_kernel).  The first finishes the matrix
+// and walks until it needs an interior cell; each later one walks inside the window refilled just before it (F_REFILL,
+// top boundary from the window's checkpoint).  Between segments the host reads back the row the walk waits for, so a
+// window the walk never enters is never refilled.
+static int32_t recompute_wave(b2a_engine* e, const FillParams& fp, const WalkParams& wp,
+                              const b2a_engine::RecomputeWave& rw, size_t wi, cudaStream_t st) {
+  const Plan& pl = e->plan;
+  const Block& k = pl.blocks[pl.waves[rw.wave].block_lo];
+  const int32_t GR = pl.G * pl.R, m = (int32_t)pl.pm[k.first];
+  const size_t row_bytes = (size_t)(k.maxn + 1) * 16;
+  // d_rcstate: WalkState at 0, EndState at 256, the segment's output at 512, the refill's task counter at 768
+  static_assert(sizeof(WalkState) <= 256 && sizeof(EndState) <= 256, "recompute scratch slots are 256 bytes");
+  uint8_t* scratch = e->d_rcstate.as<uint8_t>();
+  WalkWindow win{};
+  win.state = reinterpret_cast<WalkState*>(scratch);
+  win.es = reinterpret_cast<EndState*>(scratch + 256);
+  win.out = reinterpret_cast<int32_t*>(scratch + 512);
+  uint32_t* counter = reinterpret_cast<uint32_t*>(scratch + 768);
+  CK(cudaEventRecord(e->wave_ev[3 * wi + 0], st));
+  FillParams f1 = fp;
+  f1.tb = nullptr;
+  f1.ckpt = e->d_ckpt.as<int4>();
+  f1.win_strips = (int32_t)rw.win;
+  CK(e->shape->launch_recompute(e->flags | F_NOTB | F_CKPT, f1, f1.n_strip_tasks, e->num_sms, st, &e->last_grid, 0));
+  e->launches += 1;
+  CK(cudaEventRecord(e->wave_ev[3 * wi + 1], st));
+  const int rflags = (e->flags & (F_LUT | F_CLIPX | F_RELU)) | F_YSTREAM | F_REFILL;
+  win.first = 1;
+  win.row_lo = 1;
+  win.row_hi = 0;  // no window yet
+  uint32_t above = rw.windows;  // the walk asks for windows bottom-up, each at most once
+  for (;;) {
+    walk_window_kernel<<<1, 32, 0, st>>>(wp, win);
+    CK(cudaGetLastError());
+    e->launches += 1;
+    int32_t out[2] = {0, 0};
+    CK(cudaMemcpyAsync(out, win.out, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (out[0]) break;
+    const int32_t row = out[1];
+    const uint32_t w = (row >= 1 && row < m) ? (uint32_t)((row - 1) / GR) / rw.win : rw.windows;
+    if (w >= above)  // (the walk never increases i: an internal invariant, not a CUDA error)
+      return e->fail(B2A_E_STATE, "recomputed traceback: internal error, the walk asked for window " + std::to_string(w) +
+                                      " after window " + std::to_string(above));
+    above = w;
+    const uint32_t lo = w * rw.win, hi = std::min<uint32_t>(lo + rw.win, k.nstrips);
+    FillParams f2 = fp;
+    f2.bnd = e->d_rcbnd.as<uint8_t>();
+    f2.tb = e->d_tb.as<uint8_t>();
+    f2.strip_lo = (int32_t)lo;
+    f2.strip_hi = (int32_t)hi;
+    f2.n_strip_tasks = hi - lo;
+    f2.task_counter = counter;
+    if (w > 0) CK(cudaMemcpyAsync(f2.bnd, e->d_ckpt.as<uint8_t>() + (size_t)(w - 1) * row_bytes, row_bytes,
+                                  cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemsetAsync(counter, 0, 4, st));
+    CK(cudaMemsetAsync(f2.progress, 0, (size_t)(hi - lo) * 4, st));
+    CK(e->shape->launch_recompute(rflags, f2, hi - lo, e->num_sms, st, nullptr, 0));
+    e->launches += 1;
+    ++e->rc_filled;
+    e->rc_tb_stored += (uint64_t)(hi - lo) * strip_tb(pl, k);
+    win.first = 0;
+    win.s0 = (int32_t)lo;
+    win.row_lo = (int32_t)lo * GR + 1;
+    win.row_hi = std::min<int32_t>((int32_t)hi * GR, m - 1);
+  }
+  CK(cudaEventRecord(e->wave_ev[3 * wi + 2], st));
+  e->last_walk_warp = true;
+  return B2A_OK;
+}
+
 int32_t b2a_batch_run(b2a_engine* e) {
   if (!e) return B2A_E_INVALID;
   if (!e->staged) return e->fail(B2A_E_STATE, "b2a_batch_run before b2a_batch_stage");
@@ -750,7 +910,11 @@ int32_t b2a_batch_run(b2a_engine* e) {
   void (*const walk_warp_k)(const WalkParams) = e->score_only ? walk_warp_kernel<true> : walk_warp_kernel<false>;
   void (*const walk_lane_k)(const WalkParams) = e->score_only ? walk_kernel<true> : walk_kernel<false>;
   // pipeline slots put K2 and what follows on their high-priority stream (several waves share scratch: one stream)
-  const bool use_tail = e->is_slot && e->tail_stream != nullptr && pl.waves.size() == 1;
+  // (a recomputed wave synchronises with the host between its launches: it stays on the engine's stream)
+  const bool use_tail = e->is_slot && e->tail_stream != nullptr && pl.waves.size() == 1 && e->rc_waves.empty();
+  e->rc_filled = 0;
+  e->rc_tb_stored = 0;
+  size_t next_rc = 0;
   e->tail_used = use_tail;
   e->launches = 0;
   uint32_t* ctl = e->d_ctl.as<uint32_t>();  // [0] bad symbol, [1] walk error, [2..] per-wave task counters
@@ -840,6 +1004,12 @@ int32_t b2a_batch_run(b2a_engine* e) {
     wp.clip_len = e->d_clip.as<uint32_t>();
     wp.status = e->d_status.as<uint32_t>();
     wp.err_flag = ctl + 1;
+    if (next_rc < e->rc_waves.size() && e->rc_waves[next_rc].wave == wi) {
+      const int32_t rc = recompute_wave(e, fp, wp, e->rc_waves[next_rc++], wi, st);
+      if (rc) return rc;
+      ++wi;
+      continue;
+    }
     // (K2 inside K1's warps was slower: K2 stays its own launch)
     const bool fuse = false;
     fp.task_limit = (pl.G == 32) ? 0u : e->fill_task_limit;  // strip-pipelined tasks need the persistent grid
@@ -1093,7 +1263,7 @@ int32_t b2a_batch_fetch(b2a_engine* e, b2a_results* r, b2a_stats* stats) {
     stats->cells = e->plan.cells;
     stats->h2d_bytes = e->h2d_bytes;
     stats->d2h_bytes = d2h;
-    stats->traceback_bytes = e->plan.total_tb;
+    stats->traceback_bytes = e->plan.total_tb + e->rc_tb_stored;
     cudaEventElapsedTime(&stats->pack_ms, e->ev[0], e->ev[1]);
     for (size_t wv = 0; wv < e->plan.waves.size(); ++wv) {
       float a = 0.f, b = 0.f;
@@ -1117,7 +1287,7 @@ int32_t b2a_batch_fetch(b2a_engine* e, b2a_results* r, b2a_stats* stats) {
 static void collect_stats(b2a_engine* e, b2a_stats* stats) {
   stats->cells += e->plan.cells;
   stats->h2d_bytes += e->h2d_bytes;
-  stats->traceback_bytes += e->plan.total_tb;
+  stats->traceback_bytes += e->plan.total_tb + e->rc_tb_stored;
   float v = 0.f;
   cudaEventElapsedTime(&v, e->ev[0], e->ev[1]);
   stats->pack_ms += v;
@@ -1160,6 +1330,9 @@ static int32_t slot_finish(b2a_engine* e, b2a_engine::PipeSlot& sl, b2a_results*
   ce = cudaStreamSynchronize(c->res_stream());
   if (ce != cudaSuccess) return e->cuda_fail("pipeline: cudaStreamSynchronize", ce);
   collect_stats(c, agg);
+  e->rc_pairs += c->rc_pairs;
+  e->rc_windows += c->rc_windows;
+  e->rc_filled += c->rc_filled;
   return B2A_OK;
 }
 
@@ -1244,6 +1417,7 @@ static int32_t align_batch_pipelined(b2a_engine* e, int32_t mode, const b2a_scor
     sl.eng->tune_R = e->tune_R;
     sl.eng->walk_mode = e->walk_mode;
     sl.eng->tb_budget = e->tb_budget;
+    sl.eng->tb_recompute = e->tb_recompute;
     sl.eng->pipe_chunks = 0;
     if (sl.h_cap < nc + 1) {
       if (sl.h_opsoff) cudaFreeHost(sl.h_opsoff);
@@ -1388,6 +1562,7 @@ int32_t b2a_align_batch(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
   if (e->pipe_chunks >= 2 && results && pairs->n_pairs >= 262144) {
     e->staged = e->ran = false;
     e->score_only = false;
+    e->rc_pairs = e->rc_windows = e->rc_filled = 0;
     if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
     return align_batch_pipelined(e, mode, scoring, pairs, results, stats);
   }

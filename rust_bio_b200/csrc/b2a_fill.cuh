@@ -52,6 +52,9 @@ struct FillParams {
   uint32_t task_limit;      // 0: persistent (a warp pulls tasks until none is left); k: a warp retires after k tasks, so
                             // CTAs turn over and a higher-priority kernel's CTAs get onto the SMs (chunk pipeline)
   DevScoring sc;
+  int4* ckpt;               // F_CKPT: the checkpoint rows, [window][column] (one pair per launch)
+  int32_t win_strips;       // F_CKPT: strips per window
+  int32_t strip_lo, strip_hi;  // F_REFILL: the strips of the window, [lo, hi)
 };
 
 // Per-lane view of one warp-task (32/G pairs of one block).
@@ -84,6 +87,9 @@ struct LaneCtx {
   int32_t ge4;           // 4 * gap_extend, opaque as well (kept out of constant folding)
   uint16_t* rowm = nullptr;  // F_FINISH: block base of the row-m arena, [column][32]
   int32_t* fin = nullptr;    // F_FINISH: block base of the finish region, [field][32]
+  int4* ckpt = nullptr;      // F_CKPT: the checkpoint rows, [window][column]
+  int32_t win = 0;           // F_CKPT: strips per window
+  int32_t strip_lo = 0;      // F_REFILL: the window's first strip (c.tb holds the window's strips only)
 };
 
 // F_FINISH: column n as the lane goes down it, row after row and strip after strip (held in registers)
@@ -329,7 +335,7 @@ B2A_HD void column_step(const LaneCtx<G>& c, const int32_t j, const int32_t tste
         }
       }
     }
-    if (LAST) {
+    if (LAST && !(FLAGS & F_REFILL)) {  // (F_REFILL: column n as K2's finish left it is what the walk reads)
       const int32_t slot = (rowbase + 1 + r) * 32 + c.pi;
       if (!FIN) {
         c.rows[rows_at<G>(ROWS_SL, c.rows_pad, slot)] = s4 >> 2;
@@ -550,6 +556,10 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s, ColN& cn) {
   static_assert(!YS || G == 32, "F_YSTREAM is a warp-per-pair form");
   static_assert(!FIN || (G == 1 && !PR), "F_FINISH is a thread-per-pair form, without F_PACKREL");
   static_assert(!B8 || ((FLAGS & F_PACKTRK) != 0 && !PR), "F_BND8 needs the packed column tracker with absolute rows");
+  constexpr bool CKPT = (FLAGS & F_CKPT) != 0;
+  constexpr bool REFILL = (FLAGS & F_REFILL) != 0;
+  static_assert(!CKPT || (NOTB && G == 32 && !B8), "F_CKPT is a score-only warp-per-pair fill with 16-byte records");
+  static_assert(!REFILL || (G == 32 && !B8 && !NOTB && !TR && !TC), "F_REFILL is a warp-per-pair fill without trackers");
   constexpr int P = 32 / G;
   constexpr int TBW = tbw_of(R);
   int2* const bnd8 = reinterpret_cast<int2*>(c.bnd);
@@ -655,7 +665,11 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s, ColN& cn) {
     nyw = (n + 3) >> 2;
     if (nyw > 0) ynext = ld_yword(c, 0);
   }
-  uint4* tbs = NOTB ? nullptr : c.tb + (size_t)s * c.K * TBW * 32;
+  uint4* tbs = NOTB ? nullptr : c.tb + (size_t)(REFILL ? s - c.strip_lo : s) * c.K * TBW * 32;
+  // F_CKPT: a strip that ends a window (not the last strip) also stores its boundary row into the window's checkpoint
+  int4* const ckpt_row = (CKPT && s + 1 < c.nstrips && (s + 1) % c.win == 0)
+                             ? c.ckpt + (size_t)((s + 1) / c.win - 1) * (c.maxn + 1)
+                             : nullptr;
   const int32_t nsteps = c.K * 8;
   if (PR && TR) {
 #pragma unroll
@@ -765,6 +779,7 @@ B2A_HD void run_strip(const LaneCtx<G>& c, const int32_t s, ColN& cn) {
             }
           }
           c.bnd[bnd_index(G, j, c.pi, c.maxn)] = o;
+          if (CKPT && ckpt_row) ckpt_row[j] = o;
         }
         if (piped && ((j & 15) == 0 || j == n)) {  // publish (release) every 16 columns and at the end
           fence_device();
@@ -908,6 +923,7 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
   constexpr int FILL_WARPS = fill_warps_of(G, R);
   constexpr bool LUT = (FLAGS & F_LUT) != 0;
   constexpr int TBW = tbw_of(R);
+  constexpr bool REFILL = (FLAGS & F_REFILL) != 0;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // smem: [FILL_WARPS mbarriers (64 bytes)][LUT][per-warp staging]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
@@ -943,9 +959,10 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
       }
       b = lo;
       const uint32_t rel = task - (uint32_t)prm.blocks[b].strip_task_base;
-      const uint32_t ns = prm.blocks[b].nstrips;
+      // F_REFILL: the tasks are the strips [strip_lo, strip_hi) of each pair
+      const uint32_t ns = REFILL ? (uint32_t)(prm.strip_hi - prm.strip_lo) : prm.blocks[b].nstrips;
       sub = rel / ns;
-      only_strip = (int32_t)(rel % ns);
+      only_strip = (int32_t)(rel % ns) + (REFILL ? prm.strip_lo : 0);
     } else {
       b = task / G;
       sub = task % G;
@@ -974,7 +991,8 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
     c.ge4 = prm.ge4;
     c.only_strip = only_strip;
     c.prog_mine = strip_tasks ? prm.progress + task : nullptr;
-    c.prog_prev = (strip_tasks && only_strip > 0) ? prm.progress + task - 1 : nullptr;
+    // (F_REFILL: the window's first strip reads the seeded scratch row without waiting)
+    c.prog_prev = (strip_tasks && only_strip > (REFILL ? prm.strip_lo : 0)) ? prm.progress + task - 1 : nullptr;
     c.xs = reinterpret_cast<const uint32_t*>(stage) - xoff / 4;  // indexed by absolute row word
     c.ys = YS ? reinterpret_cast<const uint32_t*>(prm.seq + blk.seq_off + (size_t)G * xbytes + (size_t)sub * ybytes)
               : reinterpret_cast<const uint32_t*>(stage + xstage);
@@ -997,8 +1015,14 @@ __global__ void __launch_bounds__(fill_warps_of(G, R) * 32, B2A_MINB) fill_kerne
       c.rowm = reinterpret_cast<uint16_t*>(prm.rowm + blk.rowm_off);
       c.fin = prm.fin + (size_t)b * FIN_FIELDS * 32;
     }
+    if (FLAGS & F_CKPT) {
+      c.ckpt = prm.ckpt;
+      c.win = prm.win_strips;
+    }
+    c.strip_lo = REFILL ? prm.strip_lo : 0;
+    const uint32_t tb_strips = REFILL ? (uint32_t)(prm.strip_hi - prm.strip_lo) : blk.nstrips;
     c.tb = (FLAGS & F_NOTB) ? nullptr
-                            : reinterpret_cast<uint4*>(prm.tb + blk.tb_off) + (size_t)sub * blk.nstrips * blk.K * TBW * 32;
+                            : reinterpret_cast<uint4*>(prm.tb + blk.tb_off) + (size_t)sub * tb_strips * blk.K * TBW * 32;
     while (!mbar_try_wait(bar, parity)) {
     }
     parity ^= 1u;

@@ -1,13 +1,17 @@
 // One (G, R) shape of the K1 fill kernel: compile with -DB2A_G=<G> -DB2A_R=<R>.  With -DB2A_NOTB the same
 // flag cases are instantiated with F_NOTB added (score-only batches) as launch_fill_notb_<G>_<R>, in a
-// translation unit of their own so that the build stays parallel.
+// translation unit of their own so that the build stays parallel.  With -DB2A_RECOMPUTE (warp-per-pair shapes) the
+// recomputed-traceback fills are instantiated as launch_fill_recompute_<G>_<R>: the F_NOTB | F_CKPT pass over the flag
+// cases of a recomputing batch (F_PACKREL or explicit trackers, F_YSTREAM), and the tracker-free F_REFILL fills.
 #include "b2a_fill_launch.h"
 
 #ifndef B2A_G
 #error "compile with -DB2A_G=... -DB2A_R=..."
 #endif
 
-#ifdef B2A_NOTB
+#if defined(B2A_RECOMPUTE)
+#define B2A_LAUNCH_NAME launch_fill_recompute_
+#elif defined(B2A_NOTB)
 #define B2A_LAUNCH_NAME launch_fill_notb_
 #else
 #define B2A_LAUNCH_NAME launch_fill_
@@ -53,6 +57,35 @@ cudaError_t go(const FillParams& prm, uint32_t ntasks, int num_sms, cudaStream_t
 cudaError_t B2A_CAT(B2A_LAUNCH_NAME, B2A_G, B2A_R)(int flags, const FillParams& prm, uint32_t ntasks,
                                                    int num_sms, cudaStream_t stream, int* grid_out, int dry) {
   constexpr int ALL = F_TRACK_ROWS | F_TRACK_COLS | F_CLIPX;
+#if defined(B2A_RECOMPUTE)
+  static_assert(B2A_G == 32, "the recomputed traceback is a warp-per-pair form");
+#define B2A_CASE(F) case (F): return go<(F)>(prm, ntasks, num_sms, stream, grid_out, dry);
+#define B2A_PASS1(F) B2A_CASE(F_NOTB | F_CKPT | F_YSTREAM | (F))
+#define B2A_REFILL(F) B2A_CASE(F_REFILL | F_YSTREAM | (F))
+  switch (flags) {
+    B2A_PASS1(0)
+    B2A_PASS1(F_TRACK_ROWS)
+    B2A_PASS1(F_TRACK_ROWS | F_PACKREL)
+    B2A_PASS1(ALL)
+    B2A_PASS1(ALL | F_PACKREL)
+    B2A_PASS1(ALL | F_RELU)
+    B2A_PASS1(ALL | F_PACKREL | F_RELU)
+    B2A_PASS1(F_LUT)
+    B2A_PASS1(F_LUT | F_TRACK_ROWS)
+    B2A_PASS1(F_LUT | F_TRACK_ROWS | F_PACKREL)
+    B2A_PASS1(F_LUT | ALL)
+    B2A_PASS1(F_LUT | ALL | F_PACKREL)
+    B2A_PASS1(F_LUT | ALL | F_RELU)
+    B2A_PASS1(F_LUT | ALL | F_PACKREL | F_RELU)
+    B2A_REFILL(0)
+    B2A_REFILL(F_CLIPX)
+    B2A_REFILL(F_CLIPX | F_RELU)
+    B2A_REFILL(F_LUT)
+    B2A_REFILL(F_LUT | F_CLIPX)
+    B2A_REFILL(F_LUT | F_CLIPX | F_RELU)
+    default: return cudaErrorInvalidValue;
+  }
+#else
 #ifdef B2A_NOTB
   constexpr int NOTB = F_NOTB;
 #else
@@ -102,6 +135,7 @@ cudaError_t B2A_CAT(B2A_LAUNCH_NAME, B2A_G, B2A_R)(int flags, const FillParams& 
     B2A_CASE(F_LUT | ALL | F_PACKREL | F_RELU)
     default: return cudaErrorInvalidValue;
   }
+#endif
 }
 
 }  // namespace b2a

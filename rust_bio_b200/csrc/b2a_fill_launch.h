@@ -17,6 +17,8 @@ struct FillLaunch {
   FillLaunchFn launch;
   // the F_NOTB variants (score-only batches), built for the shapes choose_shape picks; null for the others
   FillLaunchFn launch_notb;
+  // the recomputed-traceback fills (F_CKPT pass and F_REFILL windows), warp-per-pair shapes only; null for the others
+  FillLaunchFn launch_recompute = nullptr;
 };
 
 #define B2A_DECLARE_FILL(G, R)                                                                  \
@@ -25,6 +27,9 @@ struct FillLaunch {
 #define B2A_DECLARE_FILL_NOTB(G, R)                                                             \
   cudaError_t launch_fill_notb_##G##_##R(int flags, const FillParams& prm, uint32_t ntasks,     \
                                          int num_sms, cudaStream_t stream, int* grid_out, int dry);
+#define B2A_DECLARE_FILL_RECOMPUTE(G, R)                                                        \
+  cudaError_t launch_fill_recompute_##G##_##R(int flags, const FillParams& prm, uint32_t ntasks, \
+                                              int num_sms, cudaStream_t stream, int* grid_out, int dry);
 
 B2A_DECLARE_FILL(1, 16)
 B2A_DECLARE_FILL(1, 8)
@@ -41,5 +46,7 @@ B2A_DECLARE_FILL_NOTB(8, 16)
 B2A_DECLARE_FILL_NOTB(8, 20)
 B2A_DECLARE_FILL_NOTB(32, 8)
 B2A_DECLARE_FILL_NOTB(32, 16)
+B2A_DECLARE_FILL_RECOMPUTE(32, 8)
+B2A_DECLARE_FILL_RECOMPUTE(32, 16)
 
 }  // namespace b2a

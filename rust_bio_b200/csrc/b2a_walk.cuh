@@ -52,6 +52,9 @@ struct WalkParams {
 };
 
 constexpr uint32_t LAZY = 15;  // "came from S of the neighbour": resolved when the walk needs it
+// windowed walk (recomputed traceback): the walker has moved onto an interior cell whose layer lies in a window that is not
+// filled yet; the layer is get_s(i, j), read once that window is
+constexpr uint32_t TB_PENDING = 14;
 
 template <class T>
 B2A_HD T ldg_ro(const T* p) {
@@ -92,6 +95,10 @@ struct PairView {
   // exact division by R and by G*R without a divide: q = (x * mul) >> 40 with mul = ceil(2^40 / d) is floor(x / d)
   // for x < 2^24 and d <= 2^10 (the walk computes a traceback address per move; sequence lengths are < 2^24)
   uint64_t mulR = 0, mulGR = 0;
+  // recomputed traceback: tb holds the strips from s0 on, and the walk reads interior cells of rows [row_lo, row_hi]
+  // only (walk_run<.., WIN>)
+  int32_t s0 = 0;
+  int32_t row_lo = 1, row_hi = 0;
   B2A_HD void set_shape(int32_t G_, int32_t R_) {
     G = G_;
     R = R_;
@@ -132,7 +139,7 @@ struct PairView {
     const int32_t lane = g * G + l;
     const int32_t t = (j - 1) + l;
     const size_t word =
-        ((((size_t)(sub * nstrips + s) * K + (t >> 3)) * TBW + (r >> 2)) * 32 + lane) * 4 + (r & 3);
+        ((((size_t)(sub * nstrips + s - s0) * K + (t >> 3)) * TBW + (r >> 2)) * 32 + lane) * 4 + (r & 3);
     return (tb[word] >> (4 * (7 - (t & 7)))) & 15u;
   }
   B2A_HD uint32_t nib_scode(uint32_t nb, int32_t i, int32_t j) const {
@@ -556,12 +563,22 @@ B2A_HD void walk_begin(const PairView& v, const EndState& es, uint8_t* ops_end, 
   w.ops_end = ops_end;
 }
 
+// WIN (recomputed traceback): whether the walker waits for the window that holds its row -- its layer is still to be
+// read from an interior cell outside [row_lo, row_hi], or it stands there on an Ins / Del layer, whose move reads the
+// cell's own nibble.  Every other read of the walk is of row m, column n, row 0, column 0 or the boundary row.
+B2A_HD bool walk_waits(const PairView& v, const int32_t i, const int32_t j, const uint32_t layer) {
+  if (i >= v.row_lo && i <= v.row_hi) return false;
+  return layer == TB_PENDING || ((layer == TB_INS || layer == TB_DEL) && i >= 1 && i < v.m && j >= 1 && j < v.n);
+}
+
 // returns true when the walk has ended (TB_START reached, or a panic path of the reference).
 // SCORES (score-only batches, K1 ran with F_NOTB and left no interior traceback): xend / yend are assigned only by the
 // suffix-clip moves, whose S-codes sit on row m (x) and column n (y) only, and the walk never increases i or j -- so
 // the walk stops as soon as it stands on a cell with i < m and j < n, before it reads that cell's layer.  Until then
 // it reads row m, column n, the boundary row and the rows arena only.  It writes no ops (ops_end may be null).
-template <bool SCORES = false>
+// WIN: a windowed walk (see walk_waits): it stops, with nothing read outside the window, where walk_waits holds.  The walk
+// never increases i, so the windows it waits for come bottom-up.
+template <bool SCORES = false, bool WIN = false>
 B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_clips, WalkState& w, int32_t max_steps) {
   const DevScoring& sc = v.sc;
   const int32_t m = v.m, n = v.n;
@@ -577,6 +594,7 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
     if (i == m) return cell_s((uint32_t)v.rowm[j * 32 + v.pi]);
     if (j == 0) return col0_sbits(sc, i);
     if (SCORES) return TB_START;  // an interior cell: the walk ends on it, its layer is never needed
+    if (WIN && (i < v.row_lo || i > v.row_hi)) return TB_PENDING;  // moved onto it; read once its window is filled
     return v.nib_scode(v.nib(i, j), i, j);
   };
   int32_t i = w.i, j = w.j;
@@ -588,6 +606,10 @@ B2A_HD bool walk_run(const PairView& v, const EndState& es, const bool filter_cl
   uint8_t* ops_end = w.ops_end;
   while (layer != TB_START && status == 0) {
     if (SCORES && i < m && j < n) break;
+    if (WIN) {
+      if (walk_waits(v, i, j, layer)) break;
+      if (layer == TB_PENDING) layer = get_s(i, j);
+    }
     if (max_steps-- <= 0) break;
     if (--guard < 0) {
       status = 1;
@@ -1130,7 +1152,7 @@ B2A_HD void prefetch_tb(const PairView& v, int32_t i, int32_t j) {
     const int32_t ln = v.g * v.G + l;
     const int32_t t = (j - 1) + l;
     const size_t word =
-        ((((size_t)(v.sub * v.nstrips + s) * v.K + (t >> 3)) * v.TBW + (r >> 2)) * 32 + ln) * 4 + (r & 3);
+        ((((size_t)(v.sub * v.nstrips + s - v.s0) * v.K + (t >> 3)) * v.TBW + (r >> 2)) * 32 + ln) * 4 + (r & 3);
     asm volatile("prefetch.global.L1 [%0];" ::"l"(v.tb + word));
   }
 #else
@@ -1231,10 +1253,8 @@ __device__ __forceinline__ void walk_lane(const WalkParams& prm, const Block& bl
   walk_store<SCORES>(prm, blk, sp, lane, cap, o);
 }
 
-// K2, one warp per pair
-template <bool SCORES>
-__device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& blk, const uint32_t b, const int pi, const int lane,
-                                          uint8_t* seq_smem) {
+// the view of pair `pi` of block `b` (warp-per-pair K2)
+__device__ __forceinline__ PairView pair_view(const WalkParams& prm, const Block& blk, const uint32_t b, const int pi) {
   const uint32_t sp = blk.first + pi;
   const int32_t P = 32 / prm.G;
   PairView v;
@@ -1263,6 +1283,16 @@ __device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& bl
   v.rows_pad = (int32_t)blk.rows_pad;
   v.rowm = reinterpret_cast<uint16_t*>(prm.rowm + blk.rowm_off);
   v.tb = reinterpret_cast<const uint32_t*>(prm.tb + blk.tb_off);
+  return v;
+}
+
+// K2, one warp per pair
+template <bool SCORES>
+__device__ __forceinline__ void walk_warp(const WalkParams& prm, const Block& blk, const uint32_t b, const int pi, const int lane,
+                                          uint8_t* seq_smem) {
+  const uint32_t sp = blk.first + pi;
+  const int32_t P = 32 / prm.G;
+  PairView v = pair_view(prm, blk, b, pi);
   if (seq_smem) {  // this warp's slice of the CTA's dynamic shared memory: x bytes, then y bytes (word granules)
     const int32_t xwn = (v.m + 3) >> 2, ywn = (v.n + 3) >> 2;
     uint32_t* xs = reinterpret_cast<uint32_t*>(seq_smem);
@@ -1295,6 +1325,58 @@ __global__ void __launch_bounds__(1024, 1) walk_warp_kernel(const WalkParams prm
   if (pi >= blk.npairs) return;
   uint8_t* mine = prm.seq_smem_per_warp ? walk_smem + (size_t)(threadIdx.x >> 5) * prm.seq_smem_per_warp : nullptr;
   walk_warp<SCORES>(prm, blk, b, (int)pi, lane, mine);
+}
+
+// K2 of a pair whose traceback is recomputed one window at a time (b2a_engine.cu, DESIGN.md §2): one warp, the pair
+// of a one-pair block.  The first segment finishes the matrix (finish_matrix_coop) and starts the walk; each segment
+// walks inside the window that was refilled last and stops where walk_waits holds, leaving its state and the row it
+// waits for in `win`; the last one stores the pair's results as walk_warp does.
+struct WalkWindow {
+  int32_t s0, row_lo, row_hi;  // the refilled window: its first strip and its rows (row_lo > row_hi: none)
+  int32_t first;               // 1: finish the matrix and begin the walk
+  WalkState* state;            // the walk between segments
+  EndState* es;
+  int32_t* out;                // [0] 1 when the walk has ended, [1] else the row it waits for
+};
+__global__ void __launch_bounds__(32, 1) walk_window_kernel(const WalkParams prm, const WalkWindow win) {
+  using C = Coop<32>;
+  const int lane = threadIdx.x & 31;
+  const Block blk = prm.blocks[0];
+  PairView v = pair_view(prm, blk, 0, 0);
+  v.s0 = win.s0;
+  v.row_lo = win.row_lo;
+  v.row_hi = win.row_hi;
+  const uint32_t cap = blk.maxm + blk.maxn + 4;
+  const bool filter_clips = prm.filter_clips != 0;
+  EndState es;
+  WalkState w;
+  if (win.first) {
+    finish_matrix_coop<32>(lane, v, es);
+    walk_begin(v, es, prm.ops_scratch + blk.ops_off + cap, w);
+  } else {
+    es = *win.es;
+    w = *win.state;
+  }
+  constexpr int32_t kBurst = 24;  // as walk_pair_coop
+  int32_t done = 0;  // 1 ended, 2 waits for another window
+  for (;;) {
+    const int32_t ci = C::from(w.i, 0) - 1 - lane, cj = C::from(w.j, 0) - 1 - lane;
+    if (ci >= v.row_lo && ci <= v.row_hi) prefetch_tb(v, ci, cj);
+    if (lane == 0) done = walk_run<false, true>(v, es, filter_clips, w, kBurst) ? 1 : (walk_waits(v, w.i, w.j, w.layer) ? 2 : 0);
+    done = C::from(done, 0);
+    if (done) break;
+  }
+  if (lane != 0) return;
+  if (done == 1) {
+    WalkOut o;
+    walk_finish(es, w, o);
+    walk_store<false>(prm, blk, blk.first, 0, cap, o);
+  } else {
+    *win.state = w;
+    *win.es = es;
+    win.out[1] = w.i;
+  }
+  win.out[0] = done == 1 ? 1 : 0;
 }
 
 template <bool SCORES>

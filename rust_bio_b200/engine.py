@@ -135,6 +135,18 @@ class Engine:
     def set_traceback_budget(self, nbytes: int):
         self._check(self._L.b2a_engine_set_traceback_budget(self._h, int(nbytes)))
 
+    def set_traceback_recompute(self, on: bool):
+        """Align a pair whose traceback is above the budget by refilling it one window of strips at a time
+        (b2a_engine_set_traceback_recompute); off by default: such a pair is refused."""
+        self._check(self._L.b2a_engine_set_traceback_recompute(self._h, 1 if on else 0))
+
+    def last_recompute(self) -> dict:
+        """Of the last full call: pairs whose traceback was recomputed, their windows, and the windows refilled
+        (b2a_engine_last_recompute)."""
+        p, w, f = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self._check(self._L.b2a_engine_last_recompute(self._h, C.byref(p), C.byref(w), C.byref(f)))
+        return {"pairs": int(p.value), "windows": int(w.value), "windows_filled": int(f.value)}
+
     @staticmethod
     def _cpairs(batch: Batch):
         blob, x_off, x_len, y_off, y_len = batch

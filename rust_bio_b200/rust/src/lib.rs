@@ -83,6 +83,9 @@ pub mod alignment {
             ) -> i32;
             fn b2a_engine_destroy(e: *mut c_void) -> i32;
             fn b2a_last_error(e: *const c_void) -> *const c_char;
+            fn b2a_engine_set_traceback_recompute(e: *mut c_void, on: i32) -> i32;
+            #[allow(dead_code)]
+            fn b2a_engine_last_recompute(e: *const c_void, pairs: *mut u64, windows: *mut u64, windows_filled: *mut u64) -> i32;
             fn b2a_align_batch(
                 e: *mut c_void,
                 mode: i32,
@@ -354,6 +357,16 @@ pub mod alignment {
                 let rc = unsafe { b2a_multi_create(&mut m, std::ptr::null(), 0) };
                 assert!(rc == 0, "b200align: cannot open every visible device (rc = {})", rc);
                 self.multi = m;
+                self
+            }
+
+            /// Align a pair whose traceback is above the engine's traceback budget (default 60 % of free HBM) by
+            /// recomputing it one window of strips at a time, instead of refusing it (not part of rust-bio's API).
+            /// Results are the same; such a pair costs at least one more fill.  Applies to this Aligner's engine;
+            /// `on_all_gpus()` batches keep each device's default.
+            pub fn with_traceback_recompute(self) -> Self {
+                let rc = unsafe { b2a_engine_set_traceback_recompute(self.engine, 1) };
+                assert!(rc == 0, "b200align: cannot set traceback recompute (rc = {})", rc);
                 self
             }
 
