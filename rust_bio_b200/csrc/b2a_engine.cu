@@ -933,6 +933,7 @@ int32_t b2a_batch_run(b2a_engine* e) {
     pk.seq = e->d_seq.as<uint8_t>();
     pk.bad_symbol = ctl;
     pk.G = pl.G;
+    pk.mapped = e->sc.alpha != 0;  // (MatchParams over more than 64 symbols compare bytes: no code map, no LUT)
     pack_kernel<<<(unsigned)pl.blocks.size(), 256, 0, st>>>(pk);
     CK(cudaGetLastError());
     ++e->launches;

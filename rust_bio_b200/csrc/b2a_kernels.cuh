@@ -20,6 +20,7 @@ struct PackParams {
   uint8_t* seq;             // staged arena
   uint32_t* bad_symbol;     // set to 1 if a byte outside the alphabet is met
   int32_t G;
+  int32_t mapped;           // codemap maps to LUT codes; 0: the identity map, where byte 0xFF is a symbol like any other
 };
 
 // K0: one CTA per block; each thread produces staged 32-bit words.
@@ -73,7 +74,7 @@ __global__ void __launch_bounds__(256) pack_kernel(const PackParams prm) {
         for (int b = 0; b < 4; ++b) {
           if ((uint32_t)b < have) {
             uint32_t code = cmap[(raw >> (8 * b)) & 0xFFu];
-            if (code == 0xFFu) {  // outside the scoring alphabet: flag it, stage a valid code
+            if (prm.mapped && code == 0xFFu) {  // outside the scoring alphabet: flag it, stage a valid code
               *prm.bad_symbol = 1u;
               code = 0;
             }
