@@ -336,7 +336,11 @@ int32_t b2a_records_decode(const void* host_records, uint32_t stride_bytes, uint
  * i.e. 64 + 40 n + ops_bytes bytes instead of n * b2a_record_stride(): short alignments (local mode on
  * reads) travel at their real length.  b2a_batch_compact_bytes waits for the batch to finish and returns the
  * segment size; ranks agree on the largest one (a MAX all-reduce of one integer), each writes its segment
- * into a buffer of that size and a single all-gather moves them. */
+ * into a buffer of that size and a single all-gather moves them.
+ * b2a_batch_compact_bytes / _into / _fixed also work after a full b2a_align_batch_banded / _hinted / _packed call:
+ * its results stay on the device until the next call on the engine, and the segment is the same.  After a banded
+ * call b2a_batch_run and b2a_batch_records* stay B2A_E_STATE (no batch is staged); after a score-only call (banded or
+ * not) the compaction is B2A_E_STATE. */
 int32_t b2a_batch_compact_bytes(b2a_engine* e, uint64_t* segment_bytes);
 int32_t b2a_batch_compact_into(b2a_engine* e, void* dev_dst, uint64_t dst_bytes);
 /* The same segment with a capacity the CALLER fixes (e.g. from the previous batch, or the bound
@@ -363,7 +367,14 @@ int32_t b2a_compact_decode(const void* host_segment, uint64_t segment_bytes, uin
  * pair list is split contiguously into equal shares, every device stages and runs its share side by side, ONE
  * ncclAllGather of the compact result segments reassembles the per-pair results on every device, and device 0's copy
  * is decoded into `results`.  Bit-identical to b2a_align_batch on one device.  Without libnccl the segments are
- * gathered onto device 0 with peer copies instead; b2a_multi_exchange_kind() names what is in use. */
+ * gathered onto device 0 with peer copies instead; b2a_multi_exchange_kind() names what is in use.
+ * A device list may name a device more than once: every entry gets its own engine and stream, no NCCL communicator is
+ * made, and the segments are peer-copied onto entry 0.  The engines of one device size their scratch independently
+ * (each from the free memory it sees: b2a_engine_set_traceback_budget), so shares that would fill a card on their own
+ * can run it out of memory (B2A_E_CUDA) together; such a list is for testing and for measuring the split on one card.
+ * A batch of fewer pairs than devices runs on device 0 alone.
+ * results->status, when set, is filled per pair as on one engine (a failing pair marks only itself); without it such
+ * a pair fails the call with the single engine's code and a "device N:" prefix on b2a_multi_last_error. */
 typedef struct b2a_multi b2a_multi;
 int32_t b2a_multi_create(b2a_multi** out, const int32_t* device_ids, int32_t n_devices);
 int32_t b2a_multi_destroy(b2a_multi* m);
@@ -372,6 +383,24 @@ const char* b2a_multi_last_error(const b2a_multi* m);
 const char* b2a_multi_exchange_kind(const b2a_multi* m);
 int32_t b2a_multi_align_batch(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
                               b2a_results* results, b2a_stats* stats);
+/* banded::Aligner over every device: each device runs b2a_align_batch_banded (hints == NULL: the k-mer matches are
+ * found on the device) or b2a_align_batch_banded_hinted on its share, then the shares are compacted, exchanged and
+ * decoded as in b2a_multi_align_batch (same segments, one collective).  Bit-identical to the single-engine call; a band
+ * above MAX_CELLS returns MIN_SCORE and no ops as there.  A hint list is checked over the whole batch before any device
+ * runs (the single engine's rules, match_off and path_off ascending): a bad one is B2A_E_INVALID. */
+int32_t b2a_multi_align_batch_banded(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, uint32_t k, uint32_t w,
+                                     const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
+                                     b2a_stats* stats);
+/* b2a_align_batch_scores and b2a_align_batch_banded_scores over every device, bit-identical to the single-engine
+ * calls and under their output rules (score, xend, yend, status; the rest NULL).  Each device writes its share
+ * straight into the caller's arrays: no ops, so no exchange. */
+int32_t b2a_multi_align_batch_scores(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
+                                     b2a_results* results, b2a_stats* stats);
+int32_t b2a_multi_align_batch_banded_scores(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, uint32_t k,
+                                            uint32_t w, const b2a_pairs* pairs, const b2a_band_hints* hints,
+                                            b2a_results* results, b2a_stats* stats);
+/* Stats of the b2a_multi_* calls: cells, h2d / d2h / traceback bytes and kernel launches are summed over the devices;
+ * pack / band / fill / walk ms and waves are the slowest device's; the fill shape fields are device 0's. */
 
 /* Measurement utility for the int32-ALU roofline (SURVEY 8d): tera lane-ops/s of
  * independent add / min-max / add+max register chains over all SMs of the device. */

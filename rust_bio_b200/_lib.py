@@ -31,7 +31,8 @@ ABI_SYMBOLS = [
     "b2a_records_decode", "b2a_batch_compact_bytes", "b2a_batch_compact_into", "b2a_compact_decode",
     "b2a_batch_compact_fixed", "b2a_gathered_fetch", "b2a_align_batch_packed", "b2a_align_batch_banded_packed",
     "b2a_multi_create", "b2a_multi_destroy", "b2a_multi_device_count", "b2a_multi_last_error",
-    "b2a_multi_exchange_kind", "b2a_multi_align_batch",
+    "b2a_multi_exchange_kind", "b2a_multi_align_batch", "b2a_multi_align_batch_banded", "b2a_multi_align_batch_scores",
+    "b2a_multi_align_batch_banded_scores",
     "b2a_util_int32_peak",
 ]
 
@@ -158,6 +159,14 @@ def load():
     L.b2a_multi_exchange_kind.restype = C.c_char_p
     L.b2a_multi_align_batch.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.POINTER(CPairs),
                                         C.POINTER(CResults), C.POINTER(CStats)]
+    L.b2a_multi_align_batch_banded.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.c_uint32, C.c_uint32,
+                                               C.POINTER(CPairs), C.POINTER(CBandHints), C.POINTER(CResults),
+                                               C.POINTER(CStats)]
+    L.b2a_multi_align_batch_scores.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.POINTER(CPairs),
+                                               C.POINTER(CResults), C.POINTER(CStats)]
+    L.b2a_multi_align_batch_banded_scores.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.c_uint32,
+                                                      C.c_uint32, C.POINTER(CPairs), C.POINTER(CBandHints),
+                                                      C.POINTER(CResults), C.POINTER(CStats)]
     L.b2a_util_int32_peak.argtypes = [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                       C.POINTER(C.c_float)]
     for name in ABI_SYMBOLS:

@@ -137,6 +137,7 @@ struct b2a_engine {
   // batch state
   bool staged = false, ran = false;
   bool score_only = false;  // staged by b2a_batch_stage_scores: F_NOTB fill, score-only K2, no ops compaction
+  bool banded_held = false;  // the last banded call's results stay on the device until the next call (compaction)
   Plan plan;
   DevScoring sc{};
   int flags = 0, mode = 0;
@@ -418,7 +419,7 @@ int32_t b2a_engine_set_tuning(b2a_engine* e, int32_t G, int32_t R) {
 static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs,
                            uint32_t& maxm, uint32_t& maxn, int64_t& score_bound) {
   if (!e || !s || !pairs) return B2A_E_INVALID;
-  e->staged = e->ran = false;
+  e->staged = e->ran = e->banded_held = false;
   e->score_only = false;
   e->rc_waves.clear();
   e->rc_pairs = e->rc_windows = e->rc_filled = 0;
@@ -1561,7 +1562,7 @@ int32_t b2a_align_batch(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
   if (!e || !scoring || !pairs) return B2A_E_INVALID;
   // large batches with host outputs: pipeline chunks so copies and planning overlap the kernels
   if (e->pipe_chunks >= 2 && results && pairs->n_pairs >= 262144) {
-    e->staged = e->ran = false;
+    e->staged = e->ran = e->banded_held = false;
     e->score_only = false;
     e->rc_pairs = e->rc_windows = e->rc_filled = 0;
     if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
@@ -2076,6 +2077,9 @@ static int32_t banded_impl(b2a_engine* e, int32_t mode, const b2a_scoring* s, ui
     stats->fill_rows_per_lane = e->strip_pairs * 2 > n ? (uint32_t)KS_R : 0u;
   }
   e->ran = false;
+  // no batch is staged (b2a_batch_run and the records stay B2A_E_STATE), but b2a_batch_compact_* can still read the
+  // call's results: d_score .. d_nops, d_clip, d_opsoff and d_opsdense are what compact_ops left above
+  e->banded_held = rc == B2A_OK;
   return rc;
 }
 
@@ -2137,7 +2141,8 @@ int32_t b2a_batch_records(b2a_engine* e, void** dev_records, uint32_t* stride_by
 
 int32_t b2a_batch_compact_bytes(b2a_engine* e, uint64_t* segment_bytes) {
   if (!e || !segment_bytes) return B2A_E_INVALID;
-  if (!e->ran) return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run");
+  if (!e->ran && !e->banded_held)
+    return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run or a banded call");
   if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to compact");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = e->n_pairs;
@@ -2152,7 +2157,8 @@ int32_t b2a_batch_compact_bytes(b2a_engine* e, uint64_t* segment_bytes) {
 
 int32_t b2a_batch_compact_into(b2a_engine* e, void* dev_dst, uint64_t dst_bytes) {
   if (!e || !dev_dst) return B2A_E_INVALID;
-  if (!e->ran) return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run");
+  if (!e->ran && !e->banded_held)
+    return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run or a banded call");
   if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to compact");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = e->n_pairs;
@@ -2187,7 +2193,8 @@ __global__ void compact_header_kernel(uint64_t* hdr, const uint64_t* ops_off, ui
 
 int32_t b2a_batch_compact_fixed(b2a_engine* e, void* dev_dst, uint64_t capacity_bytes) {
   if (!e || !dev_dst) return B2A_E_INVALID;
-  if (!e->ran) return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run");
+  if (!e->ran && !e->banded_held)
+    return e->fail(B2A_E_STATE, "compact results requested before b2a_batch_run or a banded call");
   if (e->score_only) return e->fail(B2A_E_STATE, "a score-only batch has no ops or start coordinates to compact");
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = e->n_pairs;

@@ -1,10 +1,13 @@
 // Multi-GPU form of the path behind the C ABI (SURVEY 8b / 8e): ONE process drives every visible GPU.
 //
 // The reference has no distributed layer; pairs are independent, so the batch is split contiguously over the
-// devices (equal counts), every device runs K0..K2 on its share from its own stream, and ONE ncclAllGather of
-// the compact result segments (include/b200align.h: b2a_batch_compact_*) reassembles the per-pair results on
-// every device; device 0's copy is decoded into the caller's host arrays (b2a_gathered_fetch).  The segment size
-// is agreed on the host (one process: a max over the per-device sizes, no collective).
+// devices (equal counts), every device runs its share from its own stream, and ONE ncclAllGather of the compact
+// result segments (include/b200align.h: b2a_batch_compact_*) reassembles the per-pair results on every device;
+// device 0's copy is decoded into the caller's host arrays (b2a_gathered_fetch).  The segment size is agreed on
+// the host (one process: a max over the per-device sizes, no collective).  One driver (run_split) does the split,
+// the per-device threads, the exchange and the decode for every aligner; only the job a device runs on its share
+// differs: K0..K2 (Aligner), K4 + K3 (banded::Aligner), or a score-only call whose outputs go straight to the
+// caller's host arrays (no ops, so nothing to exchange).
 //
 // NCCL is bound at run time (dlopen of libnccl.so.2: ncclCommInitAll, ncclAllGather, group calls), so the library
 // still loads on a machine without NCCL; if it cannot be found the segments are gathered onto device 0 with
@@ -16,6 +19,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
+#include <set>
 #include <string>
 #include <thread>
 #include <vector>
@@ -48,6 +53,7 @@ struct b2a_multi {
   fn_err_string err_string = nullptr;
   std::vector<nccl_comm_t> comms;
   bool use_nccl = false;
+  bool repeated = false;  // a device is listed more than once: one engine per entry, peer copies onto entry 0
   std::string err;
   int fail(int code, const std::string& what) {
     err = what;
@@ -62,6 +68,7 @@ const char* b2a_multi_last_error(const b2a_multi* m) { return m ? m->err.c_str()
 const char* b2a_multi_exchange_kind(const b2a_multi* m) {
   if (!m) return "none";
   if (m->devs.size() < 2) return "single device: no exchange";
+  if (m->repeated) return "cudaMemcpyPeerAsync onto entry 0 (a device is listed more than once: no NCCL communicator)";
   return m->use_nccl ? "ncclAllGather (libnccl.so.2, ncclCommInitAll)" : "cudaMemcpyPeerAsync onto device 0 (libnccl.so.2 not found)";
 }
 
@@ -87,10 +94,14 @@ int32_t b2a_multi_create(b2a_multi** out, const int32_t* device_ids, int32_t n_d
   int count = 0;
   if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) return B2A_E_NO_DEVICE;
   if (n_devices <= 0) n_devices = count;  // all visible devices
-  if (n_devices > count) return B2A_E_NO_DEVICE;
+  if (!device_ids && n_devices > count) return B2A_E_NO_DEVICE;
+  for (int d = 0; device_ids && d < n_devices; ++d)  // a list may repeat a device, but each must exist
+    if (device_ids[d] < 0 || device_ids[d] >= count) return B2A_E_NO_DEVICE;
   b2a_multi* m = new b2a_multi();
   for (int d = 0; d < n_devices; ++d) m->devs.push_back(device_ids ? device_ids[d] : d);
   const size_t nd = m->devs.size();
+  // ncclCommInitAll takes each device once; a list that repeats one runs every entry on its own engine and stream
+  m->repeated = std::set<int>(m->devs.begin(), m->devs.end()).size() != nd;
   m->eng.assign(nd, nullptr);
   m->streams.assign(nd, nullptr);
   m->seg_local.assign(nd, nullptr);
@@ -109,7 +120,7 @@ int32_t b2a_multi_create(b2a_multi** out, const int32_t* device_ids, int32_t n_d
     b2a_engine_set_stream(m->eng[d], m->streams[d]);
     b2a_engine_set_pipeline(m->eng[d], 0);  // shards are staged whole; the devices themselves run side by side
   }
-  if (nd > 1) {
+  if (nd > 1 && !m->repeated) {
     const char* names[] = {getenv("B2A_NCCL_PATH"), "libnccl.so.2", "libnccl.so"};
     for (const char* nm : names) {
       if (!nm || !*nm) continue;
@@ -133,15 +144,16 @@ int32_t b2a_multi_create(b2a_multi** out, const int32_t* device_ids, int32_t n_d
         }
       }
     }
-    if (!m->use_nccl) {  // peer-copy gather: device 0 must be able to read its peers
-      cudaSetDevice(m->devs[0]);
-      for (size_t d = 1; d < nd; ++d) {
-        int can = 0;
-        cudaDeviceCanAccessPeer(&can, m->devs[0], m->devs[d]);
-        if (can) cudaDeviceEnablePeerAccess(m->devs[d], 0);  // (cudaMemcpyPeerAsync works without it, through the host)
-      }
-      cudaGetLastError();
+  }
+  if (nd > 1 && !m->use_nccl) {  // peer-copy gather: device 0 must be able to read its peers
+    cudaSetDevice(m->devs[0]);
+    for (size_t d = 1; d < nd; ++d) {
+      if (m->devs[d] == m->devs[0]) continue;
+      int can = 0;
+      cudaDeviceCanAccessPeer(&can, m->devs[0], m->devs[d]);
+      if (can) cudaDeviceEnablePeerAccess(m->devs[d], 0);  // (cudaMemcpyPeerAsync works without it, through the host)
     }
+    cudaGetLastError();
   }
   *out = m;
   return B2A_OK;
@@ -149,38 +161,90 @@ int32_t b2a_multi_create(b2a_multi** out, const int32_t* device_ids, int32_t n_d
 
 int32_t b2a_multi_device_count(const b2a_multi* m) { return m ? (int32_t)m->devs.size() : 0; }
 
-int32_t b2a_multi_align_batch(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
-                              b2a_results* results, b2a_stats* stats) {
-  if (!m || !scoring || !pairs || !results) return B2A_E_INVALID;
+}  // extern "C"
+
+namespace {
+
+// One device's share of a batch: pairs [lo, hi) of the caller's list, over the part of the blob they use.
+struct Share {
+  uint64_t lo = 0, hi = 0;
+  std::vector<uint64_t> xoff, yoff;
+  b2a_pairs pairs{};
+};
+
+// What an engine runs on the whole batch (fewer pairs than devices) or on one share; a share job leaves a full
+// result on its engine when the driver exchanges (b2a_batch_compact_*), else it has written the caller's arrays.
+typedef std::function<int32_t(b2a_engine*)> WholeJob;
+typedef std::function<int32_t(b2a_engine*, const Share&, b2a_stats*)> ShareJob;
+
+// the per-pair status array of a share: a b2a_results holding only status + lo (NULL without a status array, so a
+// failing pair still fails the call as on one engine)
+b2a_results status_slice(const b2a_results* r, uint64_t lo) {
+  b2a_results s{};
+  if (r && r->status) s.status = r->status + lo;
+  return s;
+}
+
+// Cells, bytes and launches add up over the devices; kernel times and waves are the slowest device's; the shape
+// fields are device 0's.
+void merge_stats(const std::vector<b2a_stats>& ds, uint64_t exchange_d2h, b2a_stats* out) {
+  std::memset(out, 0, sizeof(*out));
+  for (const b2a_stats& s : ds) {
+    out->cells += s.cells;
+    out->h2d_bytes += s.h2d_bytes;
+    out->d2h_bytes += s.d2h_bytes;
+    out->traceback_bytes += s.traceback_bytes;
+    out->pack_ms = std::max(out->pack_ms, s.pack_ms);
+    out->fill_ms = std::max(out->fill_ms, s.fill_ms);
+    out->walk_ms = std::max(out->walk_ms, s.walk_ms);
+    out->band_ms = std::max(out->band_ms, s.band_ms);
+    out->kernel_launches += s.kernel_launches;
+    out->waves = std::max(out->waves, s.waves);
+  }
+  out->d2h_bytes += exchange_d2h;
+  out->fill_lanes_per_pair = ds[0].fill_lanes_per_pair;
+  out->fill_rows_per_lane = ds[0].fill_rows_per_lane;
+}
+
+// The one multi-GPU driver.  A batch of fewer pairs than devices runs `whole` on device 0.  Otherwise the pair list
+// is split contiguously into equal counts and every device runs `job` on its share from its own thread; with
+// `exchange` each device's result is compacted into a segment, the segments are all-gathered (or peer-copied onto
+// entry 0) and device 0's copy is decoded into `results`.  Per-pair statuses travel outside the segments: each job
+// fetched its own slice of results->status.
+int32_t run_split(b2a_multi* m, const b2a_pairs* pairs, b2a_results* results, b2a_stats* stats, bool exchange,
+                  const WholeJob& whole, const ShareJob& job) {
   const size_t nd = m->devs.size();
   const uint64_t n = pairs->n_pairs;
   if (nd == 1 || n < nd) {
     cudaSetDevice(m->devs[0]);
-    const int rc = b2a_align_batch(m->eng[0], mode, scoring, pairs, results, stats);
+    const int rc = whole(m->eng[0]);
     if (rc) m->err = b2a_last_error(m->eng[0]);
     return rc;
   }
   // contiguous split with equal counts (SURVEY 8e)
   const uint64_t per = (n + nd - 1) / nd;
-  std::vector<uint64_t> lo(nd), hi(nd), seg_bytes(nd, 0);
+  std::vector<Share> sh(nd);
+  std::vector<uint64_t> seg_bytes(nd, 0);
   std::vector<int> rcs(nd, B2A_OK);
+  std::vector<char> bad_range(nd, 0);
   std::vector<b2a_stats> dstats(nd);
-  std::vector<std::vector<uint64_t>> xoff(nd), yoff(nd);
   for (size_t d = 0; d < nd; ++d) {
-    lo[d] = std::min<uint64_t>(n, d * per);
-    hi[d] = std::min<uint64_t>(n, lo[d] + per);
+    sh[d].lo = std::min<uint64_t>(n, d * per);
+    sh[d].hi = std::min<uint64_t>(n, sh[d].lo + per);
   }
-  // every device: stage (H2D of its shard) + run + the size of its result segment, side by side
+  // every device: its share (H2D, kernels, fetch) and the size of its result segment, side by side
   {
     std::vector<std::thread> pool;
     for (size_t d = 0; d < nd; ++d) {
       pool.emplace_back([&, d]() {
         cudaSetDevice(m->devs[d]);
-        const uint64_t nc = hi[d] - lo[d];
+        Share& s = sh[d];
+        const uint64_t nc = s.hi - s.lo;
         uint64_t bmin = ~0ull, bmax = 0;
-        for (uint64_t p = lo[d]; p < hi[d]; ++p) {
+        for (uint64_t p = s.lo; p < s.hi; ++p) {
           const uint64_t bb = pairs->blob_bytes, xo = pairs->x_off[p], yo = pairs->y_off[p];
           if (xo > bb || pairs->x_len[p] > bb - xo || yo > bb || pairs->y_len[p] > bb - yo) {
+            bad_range[d] = 1;
             rcs[d] = B2A_E_INVALID;
             return;
           }
@@ -188,27 +252,29 @@ int32_t b2a_multi_align_batch(b2a_multi* m, int32_t mode, const b2a_scoring* sco
           bmax = std::max(bmax, std::max(xo + pairs->x_len[p], yo + pairs->y_len[p]));
         }
         if (bmin > bmax) bmin = bmax = 0;
-        xoff[d].resize(nc);
-        yoff[d].resize(nc);
+        s.xoff.resize(nc);
+        s.yoff.resize(nc);
         for (uint64_t i = 0; i < nc; ++i) {
-          xoff[d][i] = pairs->x_off[lo[d] + i] - bmin;
-          yoff[d][i] = pairs->y_off[lo[d] + i] - bmin;
+          s.xoff[i] = pairs->x_off[s.lo + i] - bmin;
+          s.yoff[i] = pairs->y_off[s.lo + i] - bmin;
         }
-        b2a_pairs sub{pairs->seq_blob + bmin, xoff[d].data(), pairs->x_len + lo[d], yoff[d].data(), pairs->y_len + lo[d],
-                      bmax - bmin, nc};
-        int rc = b2a_batch_stage(m->eng[d], mode, scoring, &sub);
-        if (rc == B2A_OK) rc = b2a_batch_run(m->eng[d]);
-        if (rc == B2A_OK) rc = b2a_batch_fetch(m->eng[d], nullptr, &dstats[d]);  // waits; reports a failing pair
-        if (rc == B2A_OK) rc = b2a_batch_compact_bytes(m->eng[d], &seg_bytes[d]);
+        s.pairs = b2a_pairs{pairs->seq_blob + bmin, s.xoff.data(), pairs->x_len + s.lo, s.yoff.data(),
+                            pairs->y_len + s.lo, bmax - bmin, nc};
+        int rc = job(m->eng[d], s, &dstats[d]);
+        if (rc == B2A_OK && exchange) rc = b2a_batch_compact_bytes(m->eng[d], &seg_bytes[d]);
         rcs[d] = rc;
       });
     }
     for (auto& t : pool) t.join();
   }
   for (size_t d = 0; d < nd; ++d)
-    if (rcs[d]) return m->fail(rcs[d], rcs[d] == B2A_E_INVALID && !*b2a_last_error(m->eng[d])
-                                          ? std::string("sequence offset/length outside seq_blob")
-                                          : std::string("device ") + std::to_string(m->devs[d]) + ": " + b2a_last_error(m->eng[d]));
+    if (rcs[d]) return m->fail(rcs[d], bad_range[d] ? std::string("sequence offset/length outside seq_blob")
+                                                    : std::string("device ") + std::to_string(m->devs[d]) + ": " +
+                                                          b2a_last_error(m->eng[d]));
+  if (!exchange) {  // the jobs wrote the caller's host arrays themselves
+    if (stats) merge_stats(dstats, 0, stats);
+    return B2A_OK;
+  }
   uint64_t seg = 0;
   for (uint64_t v : seg_bytes) seg = std::max(seg, v);
   seg = (seg + 255) & ~255ull;
@@ -258,30 +324,147 @@ int32_t b2a_multi_align_batch(b2a_multi* m, int32_t mode, const b2a_scoring* sco
   }
   cudaSetDevice(m->devs[0]);
   uint64_t got = 0, d2h = 0;
-  int rc = b2a_gathered_fetch(m->eng[0], m->seg_all[0], seg, (uint32_t)nd, results, &got, &d2h);
+  b2a_results body = *results;
+  body.status = nullptr;  // the jobs fetched the statuses; the segments carry none
+  int rc = b2a_gathered_fetch(m->eng[0], m->seg_all[0], seg, (uint32_t)nd, &body, &got, &d2h);
   if (rc) return m->fail(rc, b2a_last_error(m->eng[0]));
   if (got != n) return m->fail(B2A_E_STATE, "gathered segments do not hold the whole batch");
   for (size_t d = 1; d < nd; ++d) {  // the other devices' gathers finish before their buffers are reused
     cudaSetDevice(m->devs[d]);
     cudaStreamSynchronize(m->streams[d]);
   }
-  if (stats) {
-    std::memset(stats, 0, sizeof(*stats));
-    for (size_t d = 0; d < nd; ++d) {
-      stats->cells += dstats[d].cells;
-      stats->h2d_bytes += dstats[d].h2d_bytes;
-      stats->traceback_bytes += dstats[d].traceback_bytes;
-      stats->pack_ms = std::max(stats->pack_ms, dstats[d].pack_ms);
-      stats->fill_ms = std::max(stats->fill_ms, dstats[d].fill_ms);
-      stats->walk_ms = std::max(stats->walk_ms, dstats[d].walk_ms);
-      stats->kernel_launches += dstats[d].kernel_launches;
-      stats->waves = std::max(stats->waves, dstats[d].waves);
-    }
-    stats->d2h_bytes = d2h;
-    stats->fill_lanes_per_pair = dstats[0].fill_lanes_per_pair;
-    stats->fill_rows_per_lane = dstats[0].fill_rows_per_lane;
+  if (stats) merge_stats(dstats, d2h, stats);
+  return B2A_OK;
+}
+
+// A hint list is outside input: the rules of the single engine's check, and match_off / path_off ascending over
+// the whole batch, hold before anything is sliced (a share's pointers are built from these offsets).
+int32_t check_hints(b2a_multi* m, const b2a_pairs* pairs, const b2a_band_hints* h) {
+  const uint64_t n = pairs->n_pairs;
+  if (!h->match_off || (!h->match_xy && n && h->match_off[n]))
+    return m->fail(B2A_E_INVALID, "banded hints: match_off / match_xy missing");
+  if (h->path_off && (h->allowed_mismatches >= 0 || h->use_lcskpp_union))
+    return m->fail(B2A_E_INVALID, "banded hints: a match path excludes allowed_mismatches / use_lcskpp_union");
+  if (h->path_off && !h->path_idx && n && h->path_off[n]) return m->fail(B2A_E_INVALID, "banded hints: path_idx missing");
+  for (uint64_t p = 0; p < n; ++p) {
+    if (h->match_off[p + 1] < h->match_off[p]) return m->fail(B2A_E_INVALID, "banded hints: match_off not ascending");
+    if (h->path_off && h->path_off[p + 1] < h->path_off[p])
+      return m->fail(B2A_E_INVALID, "banded hints: path_off not ascending");
   }
   return B2A_OK;
+}
+
+// the hints of pairs [lo, hi): offsets rebased to the share's first pair (path indices are per pair: unchanged)
+struct HintShare {
+  std::vector<uint64_t> moff, poff;
+  b2a_band_hints h{};
+  HintShare(const b2a_band_hints* src, uint64_t lo, uint64_t hi) {
+    h = *src;
+    moff.resize(hi - lo + 1);
+    for (uint64_t p = lo; p <= hi; ++p) moff[p - lo] = src->match_off[p] - src->match_off[lo];
+    h.match_off = moff.data();
+    h.match_xy = src->match_xy ? src->match_xy + 2 * src->match_off[lo] : nullptr;
+    if (src->path_off) {
+      poff.resize(hi - lo + 1);
+      for (uint64_t p = lo; p <= hi; ++p) poff[p - lo] = src->path_off[p] - src->path_off[lo];
+      h.path_off = poff.data();
+      h.path_idx = src->path_idx ? src->path_idx + src->path_off[lo] : nullptr;
+    }
+  }
+};
+
+// score-only outputs: score, xend, yend and status, each at the share's offset; the rest must be NULL
+bool score_only_outputs_ok(b2a_multi* m, const b2a_results* r) {
+  if (r && (r->xstart || r->ystart || r->ops || r->ops_off || r->clip_len)) {
+    m->fail(B2A_E_INVALID, "a score-only batch has only score, xend, yend and status: xstart, ystart, ops, ops_off and "
+                           "clip_len must be NULL");
+    return false;
+  }
+  return true;
+}
+
+b2a_results score_slice(const b2a_results* r, uint64_t lo) {
+  b2a_results s{};
+  s.score = r->score ? r->score + lo : nullptr;
+  s.xend = r->xend ? r->xend + lo : nullptr;
+  s.yend = r->yend ? r->yend + lo : nullptr;
+  s.status = r->status ? r->status + lo : nullptr;
+  return s;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t b2a_multi_align_batch(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
+                              b2a_results* results, b2a_stats* stats) {
+  if (!m || !scoring || !pairs || !results) return B2A_E_INVALID;
+  return run_split(
+      m, pairs, results, stats, true,
+      [&](b2a_engine* e) { return b2a_align_batch(e, mode, scoring, pairs, results, stats); },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        b2a_results r = status_slice(results, s.lo);
+        int rc = b2a_batch_stage(e, mode, scoring, &s.pairs);
+        if (rc == B2A_OK) rc = b2a_batch_run(e);
+        if (rc == B2A_OK) rc = b2a_batch_fetch(e, r.status ? &r : nullptr, st);  // waits; reports a failing pair
+        return rc;
+      });
+}
+
+int32_t b2a_multi_align_batch_banded(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, uint32_t k, uint32_t w,
+                                     const b2a_pairs* pairs, const b2a_band_hints* hints, b2a_results* results,
+                                     b2a_stats* stats) {
+  if (!m || !scoring || !pairs || !results) return B2A_E_INVALID;
+  if (hints) {
+    const int rc = check_hints(m, pairs, hints);
+    if (rc) return rc;
+  }
+  return run_split(
+      m, pairs, results, stats, true,
+      [&](b2a_engine* e) {
+        return hints ? b2a_align_batch_banded_hinted(e, mode, scoring, k, w, pairs, hints, results, stats)
+                     : b2a_align_batch_banded(e, mode, scoring, k, w, pairs, results, stats);
+      },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {  // the result stays on the engine for the compaction
+        b2a_results r = status_slice(results, s.lo);
+        b2a_results* rp = r.status ? &r : nullptr;
+        if (!hints) return b2a_align_batch_banded(e, mode, scoring, k, w, &s.pairs, rp, st);
+        const HintShare hs(hints, s.lo, s.hi);
+        return b2a_align_batch_banded_hinted(e, mode, scoring, k, w, &s.pairs, &hs.h, rp, st);
+      });
+}
+
+int32_t b2a_multi_align_batch_scores(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, const b2a_pairs* pairs,
+                                     b2a_results* results, b2a_stats* stats) {
+  if (!m || !scoring || !pairs) return B2A_E_INVALID;
+  if (!score_only_outputs_ok(m, results)) return B2A_E_INVALID;
+  return run_split(
+      m, pairs, results, stats, false,
+      [&](b2a_engine* e) { return b2a_align_batch_scores(e, mode, scoring, pairs, results, stats); },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        b2a_results r = results ? score_slice(results, s.lo) : b2a_results{};
+        return b2a_align_batch_scores(e, mode, scoring, &s.pairs, results ? &r : nullptr, st);
+      });
+}
+
+int32_t b2a_multi_align_batch_banded_scores(b2a_multi* m, int32_t mode, const b2a_scoring* scoring, uint32_t k,
+                                            uint32_t w, const b2a_pairs* pairs, const b2a_band_hints* hints,
+                                            b2a_results* results, b2a_stats* stats) {
+  if (!m || !scoring || !pairs) return B2A_E_INVALID;
+  if (!score_only_outputs_ok(m, results)) return B2A_E_INVALID;
+  if (hints) {
+    const int rc = check_hints(m, pairs, hints);
+    if (rc) return rc;
+  }
+  return run_split(
+      m, pairs, results, stats, false,
+      [&](b2a_engine* e) { return b2a_align_batch_banded_scores(e, mode, scoring, k, w, pairs, hints, results, stats); },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        b2a_results r = results ? score_slice(results, s.lo) : b2a_results{};
+        if (!hints) return b2a_align_batch_banded_scores(e, mode, scoring, k, w, &s.pairs, nullptr, results ? &r : nullptr, st);
+        const HintShare hs(hints, s.lo, s.hi);
+        return b2a_align_batch_banded_scores(e, mode, scoring, k, w, &s.pairs, &hs.h, results ? &r : nullptr, st);
+      });
 }
 
 }  // extern "C"

@@ -85,7 +85,102 @@ class ScoreResults:
         return {k: getattr(self, k)[:self.n_pairs] for k in ("score", "xend", "yend", "status")}
 
 
-class Engine:
+class _BatchCalls:
+    """The batch methods Engine and MultiEngine share: host arrays in, host results out.  A subclass binds the C entry
+    points (_c_align, _c_scores, _c_banded, _c_banded_scores: the handle's calls, each returning the rc) and _check."""
+
+    @staticmethod
+    def _cpairs(batch: Batch):
+        blob, x_off, x_len, y_off, y_len = batch
+        assert blob.dtype == np.uint8 and x_off.dtype == np.uint64 and y_off.dtype == np.uint64
+        assert x_len.dtype == np.uint32 and y_len.dtype == np.uint32
+        p = lambda a: a.ctypes.data_as(C.c_void_p)
+        return CPairs(p(blob), p(x_off), p(x_len), p(y_off), p(y_len), blob.nbytes, len(x_len))
+
+    @staticmethod
+    def default_ops_capacity(batch: Batch) -> int:
+        return int(batch[2].astype(np.uint64).sum() + batch[4].astype(np.uint64).sum() + 4 * len(batch[2]))
+
+    @staticmethod
+    def _band_hints(n: int, matches, paths, allowed_mismatches, use_lcskpp_union):
+        """b2a_band_hints of per-pair match lists (and paths) -> (CBandHints, the arrays it points into)"""
+        from ._lib import CBandHints
+        if len(matches) != n or (paths is not None and len(paths) != n):
+            raise ValueError("one match list (and path) per pair")
+        moff = np.zeros(n + 1, dtype=np.uint64)
+        moff[1:] = np.cumsum([len(m) for m in matches])
+        mxy = np.array([v for m in matches for mt in m for v in mt], dtype=np.uint32).reshape(-1)
+        if mxy.size == 0:
+            mxy = np.zeros(2, dtype=np.uint32)
+        h = CBandHints(moff.ctypes.data, mxy.ctypes.data, None, None,
+                       -1 if allowed_mismatches is None else int(allowed_mismatches), 1 if use_lcskpp_union else 0)
+        keep = [moff, mxy]
+        if paths is not None:
+            poff = np.zeros(n + 1, dtype=np.uint64)
+            poff[1:] = np.cumsum([len(p) for p in paths])
+            pidx = np.array([v for p in paths for v in p] or [0], dtype=np.uint32)
+            h.path_off, h.path_idx = poff.ctypes.data, pidx.ctypes.data
+            keep += [poff, pidx]
+        return h, keep
+
+    def align_batch(self, mode: int, cscoring: CScoring, batch: Batch, results: Optional[Results] = None,
+                    ops_capacity: Optional[int] = None) -> Results:
+        """b2a_align_batch (b2a_multi_align_batch): host buffers in, host buffers out."""
+        if results is None:
+            results = Results(len(batch[2]), ops_capacity if ops_capacity is not None
+                              else self.default_ops_capacity(batch))
+        cp = self._cpairs(batch)
+        self._check(self._c_align(int(mode), C.byref(cscoring), C.byref(cp), C.byref(results.c)))
+        return results
+
+    def align_batch_scores(self, mode: int, cscoring: CScoring, batch: Batch) -> Dict[str, np.ndarray]:
+        """b2a_align_batch_scores: Alignment.score / xend / yend without the traceback -> {score, xend, yend, status}
+        (numpy, caller's pair order; a pair the reference panics on has status B2A_PAIR_PANIC)."""
+        res = ScoreResults(len(batch[2]))
+        cp = self._cpairs(batch)
+        self._check(self._c_scores(int(mode), C.byref(cscoring), C.byref(cp), C.byref(res.c)))
+        return res.as_dict()
+
+    def align_batch_banded(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch,
+                           results: Optional[Results] = None) -> Results:
+        if results is None:
+            results = Results(len(batch[2]), self.default_ops_capacity(batch))
+        cp = self._cpairs(batch)
+        self._check(self._c_banded(int(mode), C.byref(cscoring), int(k), int(w), C.byref(cp), None, C.byref(results.c)))
+        return results
+
+    def align_batch_banded_hinted(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch,
+                                  matches, paths=None, allowed_mismatches: Optional[int] = None,
+                                  use_lcskpp_union: bool = False, results: Optional[Results] = None) -> Results:
+        """banded::Aligner::custom_with_{matches, expanded_matches, match_path} over a batch
+        (b2a_align_batch_banded_hinted): matches[p] = [(xpos, ypos), ...] per pair, paths[p] = [index, ...]."""
+        n = len(batch[2])
+        h, keep = self._band_hints(n, matches, paths, allowed_mismatches, use_lcskpp_union)
+        if results is None:
+            results = Results(n, self.default_ops_capacity(batch))
+        cp = self._cpairs(batch)
+        self._check(self._c_banded(int(mode), C.byref(cscoring), int(k), int(w), C.byref(cp), C.byref(h),
+                                   C.byref(results.c)))
+        return results
+
+    def align_batch_banded_scores(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch, matches=None,
+                                  paths=None, allowed_mismatches: Optional[int] = None,
+                                  use_lcskpp_union: bool = False) -> Dict[str, np.ndarray]:
+        """b2a_align_batch_banded_scores: the banded aligner's Alignment.score / xend / yend without the traceback ->
+        {score, xend, yend, status} (numpy, caller's pair order).  matches (and paths, allowed_mismatches,
+        use_lcskpp_union) as in align_batch_banded_hinted; matches=None finds them on the device."""
+        n = len(batch[2])
+        h = keep = None
+        if matches is not None:
+            h, keep = self._band_hints(n, matches, paths, allowed_mismatches, use_lcskpp_union)
+        res = ScoreResults(n)
+        cp = self._cpairs(batch)
+        self._check(self._c_banded_scores(int(mode), C.byref(cscoring), int(k), int(w), C.byref(cp),
+                                          C.byref(h) if h is not None else None, C.byref(res.c)))
+        return res.as_dict()
+
+
+class Engine(_BatchCalls):
     def __init__(self, device: int = 0):
         self._L = _lib.load()
         h = C.c_void_p()
@@ -147,37 +242,20 @@ class Engine:
         self._check(self._L.b2a_engine_last_recompute(self._h, C.byref(p), C.byref(w), C.byref(f)))
         return {"pairs": int(p.value), "windows": int(w.value), "windows_filled": int(f.value)}
 
-    @staticmethod
-    def _cpairs(batch: Batch):
-        blob, x_off, x_len, y_off, y_len = batch
-        assert blob.dtype == np.uint8 and x_off.dtype == np.uint64 and y_off.dtype == np.uint64
-        assert x_len.dtype == np.uint32 and y_len.dtype == np.uint32
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        return CPairs(p(blob), p(x_off), p(x_len), p(y_off), p(y_len), blob.nbytes, len(x_len))
+    # the C entry points of the shared batch methods (_BatchCalls)
+    def _c_align(self, mode, cs, cp, res):
+        return self._L.b2a_align_batch(self._h, mode, cs, cp, res, C.byref(self.stats))
 
-    @staticmethod
-    def default_ops_capacity(batch: Batch) -> int:
-        return int(batch[2].astype(np.uint64).sum() + batch[4].astype(np.uint64).sum() + 4 * len(batch[2]))
+    def _c_scores(self, mode, cs, cp, res):
+        return self._L.b2a_align_batch_scores(self._h, mode, cs, cp, res, C.byref(self.stats))
 
-    def align_batch(self, mode: int, cscoring: CScoring, batch: Batch, results: Optional[Results] = None,
-                    ops_capacity: Optional[int] = None) -> Results:
-        """b2a_align_batch: host buffers in, host buffers out."""
-        if results is None:
-            results = Results(len(batch[2]), ops_capacity if ops_capacity is not None
-                              else self.default_ops_capacity(batch))
-        cp = self._cpairs(batch)
-        self._check(self._L.b2a_align_batch(self._h, int(mode), C.byref(cscoring), C.byref(cp),
-                                            C.byref(results.c), C.byref(self.stats)))
-        return results
+    def _c_banded(self, mode, cs, k, w, cp, hints, res):
+        if hints is None:
+            return self._L.b2a_align_batch_banded(self._h, mode, cs, k, w, cp, res, C.byref(self.stats))
+        return self._L.b2a_align_batch_banded_hinted(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
 
-    def align_batch_scores(self, mode: int, cscoring: CScoring, batch: Batch) -> Dict[str, np.ndarray]:
-        """b2a_align_batch_scores: Alignment.score / xend / yend without the traceback -> {score, xend, yend, status}
-        (numpy, caller's pair order; a pair the reference panics on has status B2A_PAIR_PANIC)."""
-        res = ScoreResults(len(batch[2]))
-        cp = self._cpairs(batch)
-        self._check(self._L.b2a_align_batch_scores(self._h, int(mode), C.byref(cscoring), C.byref(cp),
-                                                   C.byref(res.c), C.byref(self.stats)))
-        return res.as_dict()
+    def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
+        return self._L.b2a_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
 
     def stage_scores(self, mode: int, cscoring: CScoring, batch: Batch):
         """b2a_batch_stage_scores: stage a score-only batch (then run(), fetch_scores())."""
@@ -190,15 +268,6 @@ class Engine:
         res = ScoreResults(len(self._keep[0][2]))
         self._check(self._L.b2a_batch_fetch(self._h, C.byref(res.c), C.byref(self.stats)))
         return res.as_dict()
-
-    def align_batch_banded(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch,
-                           results: Optional[Results] = None) -> Results:
-        if results is None:
-            results = Results(len(batch[2]), self.default_ops_capacity(batch))
-        cp = self._cpairs(batch)
-        self._check(self._L.b2a_align_batch_banded(self._h, int(mode), C.byref(cscoring), int(k), int(w),
-                                                   C.byref(cp), C.byref(results.c), C.byref(self.stats)))
-        return results
 
     @staticmethod
     def pack_bitenc_pairs(pairs):
@@ -239,60 +308,6 @@ class Engine:
                                                               int(banded[1]), C.byref(pp), C.byref(results.c),
                                                               C.byref(self.stats)))
         return results
-
-    def align_batch_banded_hinted(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch,
-                                  matches, paths=None, allowed_mismatches: Optional[int] = None,
-                                  use_lcskpp_union: bool = False, results: Optional[Results] = None) -> Results:
-        """banded::Aligner::custom_with_{matches, expanded_matches, match_path} over a batch
-        (b2a_align_batch_banded_hinted): matches[p] = [(xpos, ypos), ...] per pair, paths[p] = [index, ...]."""
-        n = len(batch[2])
-        h, keep = self._band_hints(n, matches, paths, allowed_mismatches, use_lcskpp_union)
-        if results is None:
-            results = Results(n, self.default_ops_capacity(batch))
-        cp = self._cpairs(batch)
-        self._check(self._L.b2a_align_batch_banded_hinted(self._h, int(mode), C.byref(cscoring), int(k), int(w),
-                                                          C.byref(cp), C.byref(h), C.byref(results.c),
-                                                          C.byref(self.stats)))
-        return results
-
-    @staticmethod
-    def _band_hints(n: int, matches, paths, allowed_mismatches, use_lcskpp_union):
-        """b2a_band_hints of per-pair match lists (and paths) -> (CBandHints, the arrays it points into)"""
-        from ._lib import CBandHints
-        if len(matches) != n or (paths is not None and len(paths) != n):
-            raise ValueError("one match list (and path) per pair")
-        moff = np.zeros(n + 1, dtype=np.uint64)
-        moff[1:] = np.cumsum([len(m) for m in matches])
-        mxy = np.array([v for m in matches for mt in m for v in mt], dtype=np.uint32).reshape(-1)
-        if mxy.size == 0:
-            mxy = np.zeros(2, dtype=np.uint32)
-        h = CBandHints(moff.ctypes.data, mxy.ctypes.data, None, None,
-                       -1 if allowed_mismatches is None else int(allowed_mismatches), 1 if use_lcskpp_union else 0)
-        keep = [moff, mxy]
-        if paths is not None:
-            poff = np.zeros(n + 1, dtype=np.uint64)
-            poff[1:] = np.cumsum([len(p) for p in paths])
-            pidx = np.array([v for p in paths for v in p] or [0], dtype=np.uint32)
-            h.path_off, h.path_idx = poff.ctypes.data, pidx.ctypes.data
-            keep += [poff, pidx]
-        return h, keep
-
-    def align_batch_banded_scores(self, mode: int, cscoring: CScoring, k: int, w: int, batch: Batch, matches=None,
-                                  paths=None, allowed_mismatches: Optional[int] = None,
-                                  use_lcskpp_union: bool = False) -> Dict[str, np.ndarray]:
-        """b2a_align_batch_banded_scores: the banded aligner's Alignment.score / xend / yend without the traceback ->
-        {score, xend, yend, status} (numpy, caller's pair order).  matches (and paths, allowed_mismatches,
-        use_lcskpp_union) as in align_batch_banded_hinted; matches=None finds them on the device."""
-        n = len(batch[2])
-        h = keep = None
-        if matches is not None:
-            h, keep = self._band_hints(n, matches, paths, allowed_mismatches, use_lcskpp_union)
-        res = ScoreResults(n)
-        cp = self._cpairs(batch)
-        self._check(self._L.b2a_align_batch_banded_scores(self._h, int(mode), C.byref(cscoring), int(k), int(w),
-                                                          C.byref(cp), C.byref(h) if h is not None else None,
-                                                          C.byref(res.c), C.byref(self.stats)))
-        return res.as_dict()
 
     def banded_band_ranges(self, pair: int, y_len: int) -> np.ndarray:
         """Band::ranges of `pair` of the last banded call: array [y_len + 1, 2] of (start, end) row ranges."""
@@ -385,9 +400,11 @@ def default_engine(device: int = 0) -> Engine:
     return _default[device]
 
 
-class MultiEngine:
+class MultiEngine(_BatchCalls):
     """Every visible GPU from one process (b2a_multi_*): the batch is split over the devices, one ncclAllGather
-    reassembles the results, device 0's copy is returned.  Same results as Engine.align_batch."""
+    reassembles the results, device 0's copy is returned.  Same results as the Engine methods of the same names, so
+    pairwise.Aligner and banded.Aligner take one as their `engine`.  device_ids may repeat a device (one engine per
+    entry, peer copies instead of NCCL)."""
 
     def __init__(self, device_ids=None):
         self._L = _lib.load()
@@ -410,15 +427,28 @@ class MultiEngine:
     def exchange_kind(self) -> str:
         return self._L.b2a_multi_exchange_kind(self._h).decode()
 
-    def align_batch(self, mode: int, cscoring: CScoring, batch: Batch, results: Optional[Results] = None) -> Results:
-        if results is None:
-            results = Results(len(batch[2]), Engine.default_ops_capacity(batch))
-        cp = Engine._cpairs(batch)
-        rc = self._L.b2a_multi_align_batch(self._h, int(mode), C.byref(cscoring), C.byref(cp), C.byref(results.c),
-                                           C.byref(self.stats))
+    def _check(self, rc):
         if rc != 0:
             raise B2AError(rc, self._L.b2a_multi_last_error(self._h).decode())
-        return results
+
+    # the C entry points of the shared batch methods (_BatchCalls): the b2a_multi_* forms
+    def _c_align(self, mode, cs, cp, res):
+        return self._L.b2a_multi_align_batch(self._h, mode, cs, cp, res, C.byref(self.stats))
+
+    def _c_scores(self, mode, cs, cp, res):
+        return self._L.b2a_multi_align_batch_scores(self._h, mode, cs, cp, res, C.byref(self.stats))
+
+    def _c_banded(self, mode, cs, k, w, cp, hints, res):
+        return self._L.b2a_multi_align_batch_banded(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
+
+    def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
+        return self._L.b2a_multi_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
+
+    def banded_band_ranges(self, pair: int, y_len: int) -> np.ndarray:
+        """Band ranges stay on the engine of the device that aligned the pair: not available here (so
+        banded.Aligner.visualize needs an Engine)."""
+        raise NotImplementedError("band ranges are kept per device engine: banded.Aligner.visualize needs an Engine, "
+                                  "not a MultiEngine")
 
     def close(self):
         if getattr(self, "_h", None):

@@ -81,6 +81,36 @@ pub mod alignment {
                 results: *mut b2a_results,
                 stats: *mut c_void,
             ) -> i32;
+            fn b2a_multi_align_batch_banded(
+                m: *mut c_void,
+                mode: i32,
+                scoring: *const b2a_scoring,
+                k: u32,
+                w: u32,
+                pairs: *const b2a_pairs,
+                hints: *const b2a_band_hints,
+                results: *mut b2a_results,
+                stats: *mut c_void,
+            ) -> i32;
+            fn b2a_multi_align_batch_scores(
+                m: *mut c_void,
+                mode: i32,
+                scoring: *const b2a_scoring,
+                pairs: *const b2a_pairs,
+                results: *mut b2a_results,
+                stats: *mut c_void,
+            ) -> i32;
+            fn b2a_multi_align_batch_banded_scores(
+                m: *mut c_void,
+                mode: i32,
+                scoring: *const b2a_scoring,
+                k: u32,
+                w: u32,
+                pairs: *const b2a_pairs,
+                hints: *const b2a_band_hints,
+                results: *mut b2a_results,
+                stats: *mut c_void,
+            ) -> i32;
             fn b2a_engine_destroy(e: *mut c_void) -> i32;
             fn b2a_last_error(e: *const c_void) -> *const c_char;
             fn b2a_engine_set_traceback_recompute(e: *mut c_void, on: i32) -> i32;
@@ -370,6 +400,16 @@ pub mod alignment {
                 self
             }
 
+            /// Text of the last failure: of the multi-GPU handle after `on_all_gpus()`, else of the engine.
+            fn error_text(&self) -> String {
+                let p = if self.multi.is_null() {
+                    unsafe { b2a_last_error(self.engine) }
+                } else {
+                    unsafe { b2a_multi_last_error(self.multi) }
+                };
+                unsafe { CStr::from_ptr(p) }.to_string_lossy().into_owned()
+            }
+
             /// The batch in the C ABI's input layout: 16-byte aligned slots (x then y per pair), and the MatchFunc
             /// tabulated over the symbols present (mod.rs:221-228 allows any closure).
             fn pack(&self, pairs: &[(&[u8], &[u8])]) -> PackedBatch {
@@ -456,6 +496,10 @@ pub mod alignment {
                         rc
                     }
                     None => unsafe { b2a_align_batch(self.engine, mode, &cs, &cp, &mut res, std::ptr::null_mut()) },
+                    Some(BandedCall { k, w, matches: None, .. }) if !self.multi.is_null() => unsafe {
+                        b2a_multi_align_batch_banded(self.multi, mode, &cs, k, w, &cp, std::ptr::null(), &mut res,
+                                                     std::ptr::null_mut())
+                    },
                     Some(BandedCall { k, w, matches: None, .. }) => unsafe {
                         b2a_align_batch_banded(self.engine, mode, &cs, k, w, &cp, &mut res, std::ptr::null_mut())
                     },
@@ -490,13 +534,17 @@ pub mod alignment {
                             allowed_mismatches: allowed_mismatches.map(|v| v as i32).unwrap_or(-1),
                             use_lcskpp_union: use_lcskpp_union as i32,
                         };
-                        unsafe {
-                            b2a_align_batch_banded_hinted(self.engine, mode, &cs, k, w, &cp, &h, &mut res, std::ptr::null_mut())
+                        if !self.multi.is_null() {
+                            unsafe { b2a_multi_align_batch_banded(self.multi, mode, &cs, k, w, &cp, &h, &mut res, std::ptr::null_mut()) }
+                        } else {
+                            unsafe {
+                                b2a_align_batch_banded_hinted(self.engine, mode, &cs, k, w, &cp, &h, &mut res, std::ptr::null_mut())
+                            }
                         }
                     }
                 };
                 if rc != 0 {
-                    let msg = unsafe { CStr::from_ptr(b2a_last_error(self.engine)) }.to_string_lossy().into_owned();
+                    let msg = self.error_text();
                     panic!("{}", msg); // the reference panics on the same conditions (assert!, mod.rs:905)
                 }
                 let amode = match mode {
@@ -550,8 +598,9 @@ pub mod alignment {
             pub fn local_batch(&mut self, pairs: &[(&[u8], &[u8])]) -> Vec<Alignment> { self.batch(3, None, pairs) }
 
             /// Alignment::{score, xend, yend} of each pair without the traceback (b2a_align_batch_scores, or with
-            /// banded = Some((k, w)) b2a_align_batch_banded_scores), on this aligner's device.  Panics where the full
-            /// call would (a pair the reference panics on).
+            /// banded = Some((k, w)) b2a_align_batch_banded_scores), on this aligner's device, or split over every
+            /// device after `on_all_gpus()` (the b2a_multi_* forms).  Panics where the full call would (a pair the
+            /// reference panics on).
             pub(crate) fn scores_batch(&mut self, mode: i32, banded: Option<(u32, u32)>, pairs: &[(&[u8], &[u8])]) -> Vec<AlignmentScore> {
                 let n = pairs.len();
                 let pb = self.pack(pairs);
@@ -570,16 +619,23 @@ pub mod alignment {
                     clip_len: std::ptr::null_mut(),
                     status: std::ptr::null_mut(),
                 };
+                let multi = !self.multi.is_null();
                 let rc = match banded {
+                    None if multi => unsafe {
+                        b2a_multi_align_batch_scores(self.multi, mode, &cs, &cp, &mut res, std::ptr::null_mut())
+                    },
                     None => unsafe { b2a_align_batch_scores(self.engine, mode, &cs, &cp, &mut res, std::ptr::null_mut()) },
+                    Some((k, w)) if multi => unsafe {
+                        b2a_multi_align_batch_banded_scores(self.multi, mode, &cs, k, w, &cp, std::ptr::null(), &mut res,
+                                                            std::ptr::null_mut())
+                    },
                     Some((k, w)) => unsafe {
                         b2a_align_batch_banded_scores(self.engine, mode, &cs, k, w, &cp, std::ptr::null(), &mut res,
                                                       std::ptr::null_mut())
                     },
                 };
                 if rc != 0 {
-                    let msg = unsafe { CStr::from_ptr(b2a_last_error(self.engine)) }.to_string_lossy().into_owned();
-                    panic!("{}", msg);
+                    panic!("{}", self.error_text());
                 }
                 (0..n).map(|p| AlignmentScore { score: score[p], xend: xe[p] as usize, yend: ye[p] as usize }).collect()
             }
@@ -663,6 +719,12 @@ pub mod alignment {
                 }
                 pub fn with_capacity_and_scoring(m: usize, n: usize, scoring: Scoring<F>, k: usize, w: usize) -> Self {
                     Aligner { inner: super::Aligner::with_capacity_and_scoring(m, n, scoring), k, w }
+                }
+                /// Split the `*_batch` and `*_scores_batch` calls over every visible GPU (super::Aligner::on_all_gpus;
+                /// not part of rust-bio's API).  Panics if the devices cannot be opened.
+                pub fn on_all_gpus(mut self) -> Self {
+                    self.inner = self.inner.on_all_gpus();
+                    self
                 }
                 pub fn get_mut_scoring(&mut self) -> &mut Scoring<F> {
                     &mut self.inner.scoring
