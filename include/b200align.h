@@ -402,6 +402,34 @@ int32_t b2a_multi_align_batch_banded_scores(b2a_multi* m, int32_t mode, const b2
 /* Stats of the b2a_multi_* calls: cells, h2d / d2h / traceback bytes and kernel launches are summed over the devices;
  * pack / band / fill / walk ms and waves are the slowest device's; the fill shape fields are device 0's. */
 
+/* ---- bio::alignment::distance (reference src/alignment/distance.rs) over a batch of pairs: host arrays in, host arrays
+ * out, single-shot.  Input checks are the aligner's (offsets inside seq_blob, at most 2^31 - 2 pairs); a sequence may be
+ * up to 2^31 - 1 bytes.  distance[p] is pair p's result, in caller order.
+ *   b2a_levenshtein_batch, k = B2A_DIST_NONE: levenshtein(x, y) == simd::levenshtein(x, y), the unit-cost edit distance
+ *     over bytes.  Any other k: simd::bounded_levenshtein(x, y, k), i.e. the distance when it is <= min(k, max(|x|,
+ *     |y|)), else B2A_DIST_NONE (None).  Myers/Hyyro bit-parallel columns, 64 rows per word; the engine picks, per pair,
+ *     a thread with the pattern in registers (shorter side <= 256), a thread with a sliding band of words (bounded,
+ *     k <= 223), or a warp (anything else).  Results do not depend on the choice.
+ *   b2a_hamming_batch: hamming(x, y) == simd::hamming(x, y), the count of unequal positions.  A pair of unequal lengths
+ *     (the reference panics) is B2A_PAIR_PANIC in `status` with distance B2A_DIST_NONE when status is set; without a
+ *     status array it fails the call with B2A_E_INVALID.
+ * stats: cells = sum of m * n (Levenshtein; for a bounded pair too, though the band computes fewer) or of m (Hamming),
+ * pack_ms = the blob's rewrite into alphabet codes, fill_ms = the distance kernels, kernel_launches.
+ * The multi forms split the pair list over the devices as b2a_multi_align_batch_scores does; each device writes its
+ * share of distance (and status) straight into the caller's arrays.  Stats as for the other b2a_multi_* calls. */
+#define B2A_DIST_NONE 0xFFFFFFFFu
+int32_t b2a_levenshtein_batch(b2a_engine* e, uint32_t k, const b2a_pairs* pairs, uint32_t* distance, b2a_stats* stats);
+int32_t b2a_hamming_batch(b2a_engine* e, const b2a_pairs* pairs, uint32_t* distance, uint32_t* status, b2a_stats* stats);
+/* How many pairs of the last b2a_levenshtein_batch ran each way (a measurement aid; results do not depend on it):
+ * counts[0] answered on the host (an empty side, or |m - n| above the bound), counts[1..4] a thread with the pattern's
+ * 1..4 words in registers, counts[5] / counts[6] a thread with a 4- / 8-word band, counts[7] a warp.  Up to n_counts
+ * (at most 8) entries are written. */
+int32_t b2a_distance_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts);
+int32_t b2a_multi_levenshtein_batch(b2a_multi* m, uint32_t k, const b2a_pairs* pairs, uint32_t* distance,
+                                    b2a_stats* stats);
+int32_t b2a_multi_hamming_batch(b2a_multi* m, const b2a_pairs* pairs, uint32_t* distance, uint32_t* status,
+                                b2a_stats* stats);
+
 /* Measurement utility for the int32-ALU roofline (SURVEY 8d): tera lane-ops/s of
  * independent add / min-max / add+max register chains over all SMs of the device. */
 int32_t b2a_util_int32_peak(int32_t device_id, float* tops_add, float* tops_minmax, float* tops_mixed);

@@ -15,6 +15,7 @@ _VARIANT = os.environ.get("B2A_LIB_VARIANT", "")
 SO_PATH = os.path.join(HERE, "csrc", "libb200align%s.so" % (("_" + _VARIANT) if _VARIANT else ""))
 
 MIN_SCORE = -858993459
+DIST_NONE = 0xFFFFFFFF  # B2A_DIST_NONE: levenshtein without a bound; None from a bounded levenshtein
 MODE_CUSTOM, MODE_GLOBAL, MODE_SEMIGLOBAL, MODE_LOCAL = 0, 1, 2, 3
 ERRORS = {-1: "B2A_E_INVALID", -2: "B2A_E_NO_DEVICE", -3: "B2A_E_CUDA", -4: "B2A_E_RANGE",
           -5: "B2A_E_CAPACITY", -6: "B2A_E_STATE", -7: "B2A_E_UNSUPPORTED"}
@@ -33,6 +34,7 @@ ABI_SYMBOLS = [
     "b2a_multi_create", "b2a_multi_destroy", "b2a_multi_device_count", "b2a_multi_last_error",
     "b2a_multi_exchange_kind", "b2a_multi_align_batch", "b2a_multi_align_batch_banded", "b2a_multi_align_batch_scores",
     "b2a_multi_align_batch_banded_scores",
+    "b2a_levenshtein_batch", "b2a_hamming_batch", "b2a_distance_tier_pairs", "b2a_multi_levenshtein_batch", "b2a_multi_hamming_batch",
     "b2a_util_int32_peak",
 ]
 
@@ -167,6 +169,11 @@ def load():
     L.b2a_multi_align_batch_banded_scores.argtypes = [C.c_void_p, C.c_int32, C.POINTER(CScoring), C.c_uint32,
                                                       C.c_uint32, C.POINTER(CPairs), C.POINTER(CBandHints),
                                                       C.POINTER(CResults), C.POINTER(CStats)]
+    L.b2a_levenshtein_batch.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(CPairs), C.c_void_p, C.POINTER(CStats)]
+    L.b2a_hamming_batch.argtypes = [C.c_void_p, C.POINTER(CPairs), C.c_void_p, C.c_void_p, C.POINTER(CStats)]
+    L.b2a_distance_tier_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    L.b2a_multi_levenshtein_batch.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(CPairs), C.c_void_p, C.POINTER(CStats)]
+    L.b2a_multi_hamming_batch.argtypes = [C.c_void_p, C.POINTER(CPairs), C.c_void_p, C.c_void_p, C.POINTER(CStats)]
     L.b2a_util_int32_peak.argtypes = [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                       C.POINTER(C.c_float)]
     for name in ABI_SYMBOLS:

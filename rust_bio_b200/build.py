@@ -74,13 +74,19 @@ def build(force: bool = False, verbose: bool = False) -> str:
     eo = os.path.join(OBJ, "engine.o")
     objs.append(eo)
     esrc = os.path.join(CSRC, "b2a_engine.cu")
-    if force or _stale(eo, hdrs + [esrc]):
+    dist_h = os.path.join(CSRC, "b2a_distance.cuh")  # engine.o and distance.o only
+    if force or _stale(eo, hdrs + [esrc, dist_h]):
         jobs.append([NVCC, *FLAGS, "-c", esrc, "-o", eo])
     so = os.path.join(OBJ, "banded_strip_notb.o")  # the strip fill's score-only twins, beside engine.o
     objs.append(so)
     ssrc = os.path.join(CSRC, "b2a_banded_strip_notb.cu")
     if force or _stale(so, hdrs + [ssrc]):
         jobs.append([NVCC, *FLAGS, "-c", ssrc, "-o", so])
+    do = os.path.join(OBJ, "distance.o")  # the edit-distance kernels (b2a_distance.cuh: their lane logic)
+    objs.append(do)
+    dsrc = os.path.join(CSRC, "b2a_distance.cu")
+    if force or _stale(do, hdrs + [dsrc, dist_h]):
+        jobs.append([NVCC, *FLAGS, "-c", dsrc, "-o", do])
     mo = os.path.join(OBJ, "multi.o")
     objs.append(mo)
     msrc = os.path.join(CSRC, "b2a_multi.cu")

@@ -23,6 +23,7 @@
 #include "b2a_walk.cuh"
 #include "b2a_banded.cuh"
 #include "b2a_banded_strip.cuh"
+#include "b2a_distance.cuh"
 
 using namespace b2a;
 
@@ -119,6 +120,7 @@ struct b2a_engine {
   bool banded_strip = true;  // K3s: strip-wavefront fill for the pairs K4 marks (B2A_BANDED_STRIP=0: never)
   bool banded_strip_lastcol = true;  // ... also for bands reaching column n (B2A_BANDED_STRIP_LASTCOL=0: those stay with K3)
   uint64_t strip_pairs = 0;  // pairs the strip path finished in the last banded call (the rest ran the K3 loops)
+  uint64_t dist_tier_pairs[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // pairs per tier of the last b2a_levenshtein_batch (DT_*)
   // packed input (b2a_align_batch_packed): the caller's "blob" is BitEnc storage of this width (0 = bytes); the
   // engine unpacks it on the device and uses its own byte offsets (eff_xoff / eff_yoff) from then on
   uint32_t packed_width = 0;
@@ -414,6 +416,44 @@ int32_t b2a_engine_set_tuning(b2a_engine* e, int32_t G, int32_t R) {
 
 }  // extern "C"
 
+// The caller's byte blob -> d_blob (with 16 bytes of slack for the kernels' wide loads), and with `present` the byte
+// values it holds, found on the device in one flat pass (symbols_kernel).  stage_front and the distance calls.
+static int32_t upload_blob(b2a_engine* e, const b2a_pairs* pairs, bool* present) {
+  cudaStream_t st = e->stream;
+  CK(e->d_blob.reserve(pairs->blob_bytes + 16));
+  e->h2d_bytes += pairs->blob_bytes;
+  if (pairs->blob_bytes) CK(cudaMemcpyAsync(e->d_blob.p, pairs->seq_blob, pairs->blob_bytes, cudaMemcpyHostToDevice, st));
+  if (!present) return B2A_OK;
+  CK(e->d_ctl.reserve(2048));
+  uint32_t* flags = e->d_ctl.as<uint32_t>() + 256;  // 256 words
+  CK(cudaMemsetAsync(flags, 0, 1024, st));
+  if (pairs->blob_bytes) {
+    symbols_kernel<<<e->num_sms * 8, 256, 0, st>>>(e->d_blob.as<uint8_t>(), pairs->blob_bytes, flags);
+    CK(cudaGetLastError());
+  }
+  uint32_t hflags[256];
+  CK(cudaMemcpyAsync(hflags, flags, 1024, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int k = 0; k < 256; ++k) present[k] = hflags[k] != 0;
+  return B2A_OK;
+}
+
+// The batch's alphabet, ascending (one symbol at least), remembered for b2a_engine_last_alphabet.
+static std::vector<int> batch_symbols(b2a_engine* e, const bool* present) {
+  std::vector<int> syms;
+  for (int k = 0; k < 256; ++k)
+    if (present[k]) syms.push_back(k);
+  if (syms.empty()) syms.push_back(0);
+  e->last_syms.assign(syms.begin(), syms.end());
+  return syms;
+}
+
+// codemap_host: symbol a of the alphabet -> code a, every other byte -> 0xFF
+static void compact_codemap(b2a_engine* e, const std::vector<int>& syms) {
+  for (int k = 0; k < 256; ++k) e->codemap_host[k] = 0xFF;
+  for (size_t a = 0; a < syms.size(); ++a) e->codemap_host[syms[a]] = (uint8_t)a;
+}
+
 // Shared front half of a batch: validation (the reference's constructor asserts), clip presets, the
 // i32 range guard, alphabet discovery + LUT, and the upload of the caller's blob.
 static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs,
@@ -521,28 +561,12 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
     if (!(s->alphabet && s->alphabet_len))
       for (uint32_t k = 0; k < (1u << pw); ++k) present[k] = true;  // the ranks a BitEnc of this width can hold
   } else {
-    CK(e->d_blob.reserve(pairs->blob_bytes + 16));
-    CK(up(e->d_blob, pairs->seq_blob, pairs->blob_bytes));
+    rc = upload_blob(e, pairs, !(s->alphabet && s->alphabet_len) ? present : nullptr);
+    if (rc) return rc;
   }
-  if (s->alphabet && s->alphabet_len) {  // caller-supplied alphabet (tabulated MatchFunc or MatchParams alike)
+  if (s->alphabet && s->alphabet_len)  // caller-supplied alphabet (tabulated MatchFunc or MatchParams alike)
     for (uint32_t k = 0; k < s->alphabet_len; ++k) present[s->alphabet[k]] = true;
-  } else if (!pw) {
-    uint32_t* flags = e->d_ctl.as<uint32_t>() + 256;  // 256 words
-    CK(cudaMemsetAsync(flags, 0, 1024, st));
-    if (pairs->blob_bytes) {
-      symbols_kernel<<<e->num_sms * 8, 256, 0, st>>>(e->d_blob.as<uint8_t>(), pairs->blob_bytes, flags);
-      CK(cudaGetLastError());
-    }
-    uint32_t hflags[256];
-    CK(cudaMemcpyAsync(hflags, flags, 1024, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    for (int k = 0; k < 256; ++k) present[k] = hflags[k] != 0;
-  }
-  std::vector<int> syms;
-  for (int k = 0; k < 256; ++k)
-    if (present[k]) syms.push_back(k);
-  if (syms.empty()) syms.push_back(0);
-  e->last_syms.assign(syms.begin(), syms.end());
+  const std::vector<int> syms = batch_symbols(e, present);
   int64_t maxabs = std::max<int64_t>(std::llabs((long long)s->match_score), std::llabs((long long)s->mismatch_score));
   for (int k = 0; k < 256; ++k) e->codemap_host[k] = (uint8_t)k;
   e->lut_host.clear();
@@ -550,8 +574,7 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
     return e->fail(B2A_E_UNSUPPORTED, "MatchFunc table over more than 128 distinct symbols");
   if ((int)syms.size() <= (s->table ? kMaxAlphaTable : kMaxAlpha)) {
     sc.alpha = (int32_t)syms.size();
-    for (int k = 0; k < 256; ++k) e->codemap_host[k] = 0xFF;
-    for (int a = 0; a < sc.alpha; ++a) e->codemap_host[syms[a]] = (uint8_t)a;
+    compact_codemap(e, syms);
     const size_t aa = (size_t)sc.alpha * sc.alpha;
     e->lut_host.resize(aa + (size_t)lut_entries(sc.alpha));  // [plain | 4*v+3 for K1's packed domain + its poison row]
     if (s->table) maxabs = 0;
@@ -2346,6 +2369,196 @@ int32_t b2a_records_decode(const void* host_records, uint32_t stride, uint64_t n
   }
   if (r->ops_off) r->ops_off[n] = off;
   return B2A_OK;
+}
+
+}  // extern "C"
+
+// ---- batched edit distance (bio::alignment::distance): kernels and lane logic in b2a_distance.cu / .cuh
+
+// What the distance calls share before any device work: the engine's staged state is dropped (they reuse its
+// buffers), the pair count and every offset + length are checked against the blob, and the pair arrays are uploaded.
+static int32_t dist_front(b2a_engine* e, const b2a_pairs* pairs) {
+  e->staged = e->ran = e->banded_held = false;
+  e->score_only = false;
+  if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
+  const uint64_t n = pairs->n_pairs;
+  if (n > 0x7ffffffeull) return e->fail(B2A_E_INVALID, "more than 2^31 - 2 pairs in one batch");
+  for (uint64_t p = 0; p < n; ++p) {
+    const uint64_t bb = pairs->blob_bytes, xo = pairs->x_off[p], yo = pairs->y_off[p];
+    if (xo > bb || pairs->x_len[p] > bb - xo || yo > bb || pairs->y_len[p] > bb - yo)
+      return e->fail(B2A_E_INVALID, "sequence offset/length outside seq_blob");
+    if (pairs->x_len[p] > 0x7fffffffu || pairs->y_len[p] > 0x7fffffffu)
+      return e->fail(B2A_E_RANGE, "sequence longer than 2^31 - 1");
+  }
+  e->n_pairs = n;
+  e->h2d_bytes = 0;
+  e->launches = 0;
+  cudaStream_t st = e->stream;
+  CK(e->d_xoff.reserve(n * 8 + 8));
+  CK(e->d_yoff.reserve(n * 8 + 8));
+  CK(e->d_xlen.reserve(n * 4 + 4));
+  CK(e->d_ylen.reserve(n * 4 + 4));
+  CK(e->d_score.reserve(n * 4 + 4));  // the distances
+  if (n) {
+    CK(cudaMemcpyAsync(e->d_xoff.p, pairs->x_off, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->d_yoff.p, pairs->y_off, n * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->d_xlen.p, pairs->x_len, n * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->d_ylen.p, pairs->y_len, n * 4, cudaMemcpyHostToDevice, st));
+    e->h2d_bytes += n * 24;
+  }
+  return B2A_OK;
+}
+
+static DistArgs dist_args(b2a_engine* e, uint32_t k, int sigma) {
+  DistArgs a{};
+  a.codes = e->d_blob.as<uint8_t>();
+  a.x_off = e->d_xoff.as<uint64_t>();
+  a.x_len = e->d_xlen.as<uint32_t>();
+  a.y_off = e->d_yoff.as<uint64_t>();
+  a.y_len = e->d_ylen.as<uint32_t>();
+  a.k = k;
+  a.sigma = sigma;
+  a.dist = e->d_score.as<uint32_t>();
+  return a;
+}
+
+// the distances back into the caller's array, then the pairs the host answered; stats of the call
+static int32_t dist_finish(b2a_engine* e, uint32_t* distance, const std::vector<std::pair<uint64_t, uint32_t>>& done,
+                           uint64_t cells, bool timed, b2a_stats* stats) {
+  const uint64_t n = e->n_pairs;
+  cudaStream_t st = e->stream;
+  if (n) CK(cudaMemcpyAsync(distance, e->d_score.p, n * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (const auto& pv : done) distance[pv.first] = pv.second;
+  if (stats) {
+    std::memset(stats, 0, sizeof(*stats));
+    stats->cells = cells;
+    stats->h2d_bytes = e->h2d_bytes;
+    stats->d2h_bytes = n * 4;
+    if (timed) {
+      cudaEventElapsedTime(&stats->pack_ms, e->ev[0], e->ev[1]);
+      cudaEventElapsedTime(&stats->fill_ms, e->ev[1], e->ev[2]);
+    }
+    stats->kernel_launches = e->launches;
+  }
+  return B2A_OK;
+}
+
+extern "C" {
+
+int32_t b2a_levenshtein_batch(b2a_engine* e, uint32_t k, const b2a_pairs* pairs, uint32_t* distance, b2a_stats* stats) {
+  if (!e || !pairs || (!distance && pairs->n_pairs)) return B2A_E_INVALID;
+  int32_t rc = dist_front(e, pairs);
+  if (rc) return rc;
+  const uint64_t n = pairs->n_pairs;
+  cudaStream_t st = e->stream;
+  // the tier of every pair from its lengths and the bound; tasks grouped by tier, results land by pair index
+  std::vector<uint32_t> tasks[DT_COUNT];
+  std::vector<std::pair<uint64_t, uint32_t>> done;
+  uint64_t cells = 0;
+  uint32_t warp_maxn = 0;
+  for (uint64_t p = 0; p < n; ++p) {
+    const uint32_t m = pairs->x_len[p], nn = pairs->y_len[p];
+    cells += (uint64_t)m * nn;
+    uint32_t v = 0;
+    const int t = dist_tier(m, nn, k, &v);
+    if (t == DT_DONE) {
+      done.push_back({p, v});
+      continue;
+    }
+    tasks[t].push_back((uint32_t)p);
+    if (t == DT_WARP) warp_maxn = std::max(warp_maxn, std::max(m, nn));
+  }
+  const uint64_t n_dp = n - done.size();
+  e->dist_tier_pairs[DT_DONE] = done.size();
+  for (int t = 1; t < DT_COUNT; ++t) e->dist_tier_pairs[t] = tasks[t].size();
+  if (n_dp) {
+    // the blob as codes of the batch's alphabet: the match masks are sigma words per pattern word
+    bool present[256];
+    rc = upload_blob(e, pairs, present);
+    if (rc) return rc;
+    const std::vector<int> syms = batch_symbols(e, present);
+    compact_codemap(e, syms);
+    CK(e->d_codemap.reserve(256));
+    CK(cudaMemcpyAsync(e->d_codemap.p, e->codemap_host, 256, cudaMemcpyHostToDevice, st));
+    std::vector<uint32_t> all;
+    all.reserve(n_dp);
+    for (int t = 1; t < DT_COUNT; ++t) all.insert(all.end(), tasks[t].begin(), tasks[t].end());
+    CK(e->d_order.reserve(all.size() * 4 + 4));
+    CK(cudaMemcpyAsync(e->d_order.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice, st));
+    CK(e->d_ctl.reserve(2048));
+    CK(cudaMemsetAsync(e->d_ctl.p, 0, 4, st));  // the warp tier's pair counter
+    e->h2d_bytes += 256 + all.size() * 4;
+    const int sigma = (int)syms.size();
+    int ctas = 0, wpc = 0;
+    const uint64_t bnd_words = ((uint64_t)warp_maxn + 15) / 16;
+    if (!tasks[DT_WARP].empty()) {
+      CK(lev_warp_grid(sigma, e->num_sms, (uint32_t)tasks[DT_WARP].size(), &ctas, &wpc));
+      CK(e->d_bnd.reserve((uint64_t)ctas * wpc * bnd_words * 4 + 16));
+    }
+    CK(cudaEventRecord(e->ev[0], st));
+    CK(launch_dist_translate(e->d_blob.as<uint8_t>(), pairs->blob_bytes, e->d_codemap.as<uint8_t>(), e->num_sms, st));
+    ++e->launches;
+    CK(cudaEventRecord(e->ev[1], st));
+    DistArgs a = dist_args(e, k, sigma);
+    uint64_t at = 0;
+    for (int t = 1; t < DT_COUNT; ++t) {
+      a.tasks = e->d_order.as<uint32_t>() + at;
+      a.n_tasks = (uint32_t)tasks[t].size();
+      at += tasks[t].size();
+      if (!a.n_tasks) continue;
+      if (t == DT_WARP)
+        CK(launch_lev_warp(a, ctas, wpc, e->d_bnd.as<uint32_t>(), bnd_words, e->d_ctl.as<uint32_t>(), st));
+      else
+        CK(launch_lev_thread(t, a, st));
+      ++e->launches;
+    }
+    CK(cudaEventRecord(e->ev[2], st));
+  }
+  return dist_finish(e, distance, done, cells, n_dp != 0, stats);
+}
+
+int32_t b2a_distance_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts) {
+  if (!e || (!counts && n_counts)) return B2A_E_INVALID;
+  static_assert(DT_COUNT == 8, "b2a_distance_tier_pairs reports eight tiers");
+  for (uint32_t t = 0; t < n_counts && t < (uint32_t)DT_COUNT; ++t) counts[t] = e->dist_tier_pairs[t];
+  return B2A_OK;
+}
+
+int32_t b2a_hamming_batch(b2a_engine* e, const b2a_pairs* pairs, uint32_t* distance, uint32_t* status,
+                          b2a_stats* stats) {
+  if (!e || !pairs || (!distance && pairs->n_pairs)) return B2A_E_INVALID;
+  int32_t rc = dist_front(e, pairs);  // (a refused batch leaves status untouched)
+  if (rc) return rc;
+  const uint64_t n = pairs->n_pairs;
+  // unequal lengths: the reference panics (distance.rs); only that pair when there is a status array
+  std::vector<std::pair<uint64_t, uint32_t>> done;
+  uint64_t cells = 0;
+  for (uint64_t p = 0; p < n; ++p) {
+    const uint32_t m = pairs->x_len[p], nn = pairs->y_len[p];
+    if (m != nn) {
+      if (!status)
+        return e->fail(B2A_E_INVALID, "pair " + std::to_string(p) +
+                                          ": hamming distance cannot be calculated for texts of different length (" +
+                                          std::to_string(m) + "!=" + std::to_string(nn) + ")");
+      done.push_back({p, DIST_NONE});
+    } else {
+      cells += m;
+    }
+  }
+  if (status)
+    for (uint64_t p = 0; p < n; ++p) status[p] = pairs->x_len[p] != pairs->y_len[p] ? B2A_PAIR_PANIC : B2A_PAIR_OK;
+  cudaStream_t st = e->stream;
+  rc = upload_blob(e, pairs, nullptr);
+  if (rc) return rc;
+  CK(cudaEventRecord(e->ev[0], st));
+  CK(cudaEventRecord(e->ev[1], st));
+  if (n) {
+    CK(launch_hamming(dist_args(e, 0, 256), n, e->num_sms, st));
+    ++e->launches;
+  }
+  CK(cudaEventRecord(e->ev[2], st));
+  return dist_finish(e, distance, done, cells, true, stats);
 }
 
 }  // extern "C"

@@ -467,4 +467,39 @@ int32_t b2a_multi_align_batch_banded_scores(b2a_multi* m, int32_t mode, const b2
       });
 }
 
+int32_t b2a_multi_levenshtein_batch(b2a_multi* m, uint32_t k, const b2a_pairs* pairs, uint32_t* distance,
+                                    b2a_stats* stats) {
+  if (!m || !pairs || (!distance && pairs->n_pairs)) return B2A_E_INVALID;
+  return run_split(
+      m, pairs, nullptr, stats, false, [&](b2a_engine* e) { return b2a_levenshtein_batch(e, k, pairs, distance, stats); },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        return b2a_levenshtein_batch(e, k, &s.pairs, distance + s.lo, st);
+      });
+}
+
+int32_t b2a_multi_hamming_batch(b2a_multi* m, const b2a_pairs* pairs, uint32_t* distance, uint32_t* status,
+                                b2a_stats* stats) {
+  if (!m || !pairs || (!distance && pairs->n_pairs)) return B2A_E_INVALID;
+  if (!status && m->devs.size() > 1) {
+    // a pair of unequal lengths fails the call; a share would name it by its index in the share, so the whole batch
+    // is checked here first (offsets, then lengths, in the single engine's order) and the caller's index reported
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p) {
+      const uint64_t bb = pairs->blob_bytes, xo = pairs->x_off[p], yo = pairs->y_off[p];
+      if (xo > bb || pairs->x_len[p] > bb - xo || yo > bb || pairs->y_len[p] > bb - yo)
+        return m->fail(B2A_E_INVALID, "sequence offset/length outside seq_blob");
+    }
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p)
+      if (pairs->x_len[p] != pairs->y_len[p])
+        return m->fail(B2A_E_INVALID, "pair " + std::to_string(p) +
+                                          ": hamming distance cannot be calculated for texts of different length (" +
+                                          std::to_string(pairs->x_len[p]) + "!=" + std::to_string(pairs->y_len[p]) + ")");
+  }
+  return run_split(
+      m, pairs, nullptr, stats, false,
+      [&](b2a_engine* e) { return b2a_hamming_batch(e, pairs, distance, status, stats); },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        return b2a_hamming_batch(e, &s.pairs, distance + s.lo, status ? status + s.lo : nullptr, st);
+      });
+}
+
 }  // extern "C"

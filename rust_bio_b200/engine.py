@@ -87,7 +87,7 @@ class ScoreResults:
 
 class _BatchCalls:
     """The batch methods Engine and MultiEngine share: host arrays in, host results out.  A subclass binds the C entry
-    points (_c_align, _c_scores, _c_banded, _c_banded_scores: the handle's calls, each returning the rc) and _check."""
+    points (_c_align, _c_scores, _c_banded, _c_banded_scores, _c_levenshtein, _c_hamming: the handle's calls, each returning the rc) and _check."""
 
     @staticmethod
     def _cpairs(batch: Batch):
@@ -179,6 +179,29 @@ class _BatchCalls:
                                           C.byref(h) if h is not None else None, C.byref(res.c)))
         return res.as_dict()
 
+    def levenshtein_batch(self, batch: Batch, k: Optional[int] = None) -> np.ndarray:
+        """b2a_levenshtein_batch: per pair, levenshtein(x, y) (k=None), or simd::bounded_levenshtein(x, y, k) with
+        None as DIST_NONE -> uint32 numpy array in the caller's pair order."""
+        kk = _lib.DIST_NONE if k is None else int(k)
+        if not 0 <= kk <= _lib.DIST_NONE:
+            raise ValueError("k must fit in u32")
+        out = np.zeros(max(1, len(batch[2])), dtype=np.uint32)
+        cp = self._cpairs(batch)
+        self._check(self._c_levenshtein(kk, C.byref(cp), out.ctypes.data_as(C.c_void_p)))
+        return out[:len(batch[2])]
+
+    def hamming_batch(self, batch: Batch, pair_status: bool = True):
+        """b2a_hamming_batch: per pair, hamming(x, y) -> (uint32 distances, uint32 B2A_PAIR_* statuses); a pair of
+        unequal lengths is B2A_PAIR_PANIC with distance DIST_NONE.  pair_status=False: such a pair fails the call
+        (B2AError) and only the distances are returned."""
+        n = len(batch[2])
+        out = np.zeros(max(1, n), dtype=np.uint32)
+        st = np.zeros(max(1, n), dtype=np.uint32) if pair_status else None
+        cp = self._cpairs(batch)
+        self._check(self._c_hamming(C.byref(cp), out.ctypes.data_as(C.c_void_p),
+                                    st.ctypes.data_as(C.c_void_p) if pair_status else None))
+        return (out[:n], st[:n]) if pair_status else out[:n]
+
 
 class Engine(_BatchCalls):
     def __init__(self, device: int = 0):
@@ -242,6 +265,13 @@ class Engine(_BatchCalls):
         self._check(self._L.b2a_engine_last_recompute(self._h, C.byref(p), C.byref(w), C.byref(f)))
         return {"pairs": int(p.value), "windows": int(w.value), "windows_filled": int(f.value)}
 
+    def distance_tier_pairs(self) -> list:
+        """Pairs of the last levenshtein_batch per tier: [host-answered, register tier with 1..4 words (4 entries),
+        4-word band, 8-word band, warp] (b2a_distance_tier_pairs; a measurement aid)."""
+        buf = np.zeros(8, dtype=np.uint64)
+        self._check(self._L.b2a_distance_tier_pairs(self._h, buf.ctypes.data_as(C.c_void_p), 8))
+        return [int(v) for v in buf]
+
     # the C entry points of the shared batch methods (_BatchCalls)
     def _c_align(self, mode, cs, cp, res):
         return self._L.b2a_align_batch(self._h, mode, cs, cp, res, C.byref(self.stats))
@@ -253,6 +283,12 @@ class Engine(_BatchCalls):
         if hints is None:
             return self._L.b2a_align_batch_banded(self._h, mode, cs, k, w, cp, res, C.byref(self.stats))
         return self._L.b2a_align_batch_banded_hinted(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
+
+    def _c_levenshtein(self, k, cp, out):
+        return self._L.b2a_levenshtein_batch(self._h, k, cp, out, C.byref(self.stats))
+
+    def _c_hamming(self, cp, out, status):
+        return self._L.b2a_hamming_batch(self._h, cp, out, status, C.byref(self.stats))
 
     def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
@@ -440,6 +476,12 @@ class MultiEngine(_BatchCalls):
 
     def _c_banded(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_multi_align_batch_banded(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
+
+    def _c_levenshtein(self, k, cp, out):
+        return self._L.b2a_multi_levenshtein_batch(self._h, k, cp, out, C.byref(self.stats))
+
+    def _c_hamming(self, cp, out, status):
+        return self._L.b2a_multi_hamming_batch(self._h, cp, out, status, C.byref(self.stats))
 
     def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_multi_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))

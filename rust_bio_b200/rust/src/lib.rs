@@ -1,4 +1,4 @@
-//! `bio_b200::alignment::pairwise` -- the rust-bio 4.0.1 pairwise API on an H100.
+//! `bio_b200::alignment::{pairwise, distance}` -- the rust-bio 4.0.1 pairwise and distance APIs on an H100.
 //!
 //! NOT COMPILED BY THIS REPOSITORY'S BUILD (it needs no Rust toolchain).  It is the binding a
 //! maintainer adds next to `bio`: same type and method names as
@@ -790,6 +790,188 @@ pub mod alignment {
                     c.paths = Some(paths);
                     self.inner.batch(0, Some(c), pairs)
                 }
+            }
+        }
+    }
+
+    // ---------------------------------------------------------------- distance, reference src/alignment/distance.rs
+    /// `bio::alignment::distance` on the GPU: the reference's free functions (each a batch of one) and `*_batch`
+    /// forms over a pair list, all on this thread's engine on device 0 (created on first use).
+    pub mod distance {
+        use std::cell::RefCell;
+        use std::ffi::CStr;
+        use std::os::raw::{c_char, c_void};
+
+        /// B2A_DIST_NONE (include/b200align.h): no bound (k), or None (a bounded result)
+        const DIST_NONE: u32 = 0xFFFF_FFFF;
+        const PAIR_OK: u32 = 0;
+
+        #[repr(C)]
+        struct b2a_pairs {
+            seq_blob: *const u8,
+            x_off: *const u64,
+            x_len: *const u32,
+            y_off: *const u64,
+            y_len: *const u32,
+            blob_bytes: u64,
+            n_pairs: u64,
+        }
+        #[link(name = "b200align")]
+        extern "C" {
+            fn b2a_engine_create(out: *mut *mut c_void, device_id: i32) -> i32;
+            fn b2a_engine_destroy(e: *mut c_void) -> i32;
+            fn b2a_last_error(e: *const c_void) -> *const c_char;
+            fn b2a_levenshtein_batch(e: *mut c_void, k: u32, pairs: *const b2a_pairs, distance: *mut u32,
+                                     stats: *mut c_void) -> i32;
+            fn b2a_hamming_batch(e: *mut c_void, pairs: *const b2a_pairs, distance: *mut u32, status: *mut u32,
+                                 stats: *mut c_void) -> i32;
+        }
+
+        struct Engine(*mut c_void);
+        impl Drop for Engine {
+            fn drop(&mut self) {
+                if !self.0.is_null() {
+                    unsafe { b2a_engine_destroy(self.0) };
+                }
+            }
+        }
+        thread_local! {
+            static ENGINE: RefCell<Engine> = RefCell::new(Engine(std::ptr::null_mut()));
+        }
+
+        /// The pairs back to back in one blob (the kernels take any offsets)
+        struct Batch {
+            blob: Vec<u8>,
+            x_off: Vec<u64>,
+            y_off: Vec<u64>,
+            x_len: Vec<u32>,
+            y_len: Vec<u32>,
+        }
+        impl Batch {
+            fn new(pairs: &[(&[u8], &[u8])]) -> Self {
+                let mut b = Batch { blob: Vec::new(), x_off: Vec::new(), y_off: Vec::new(), x_len: Vec::new(), y_len: Vec::new() };
+                for (x, y) in pairs {
+                    assert!(x.len() < (1usize << 31) && y.len() < (1usize << 31), "b200align: a sequence longer than 2^31 - 1");
+                    b.x_off.push(b.blob.len() as u64);
+                    b.blob.extend_from_slice(x);
+                    b.y_off.push(b.blob.len() as u64);
+                    b.blob.extend_from_slice(y);
+                    b.x_len.push(x.len() as u32);
+                    b.y_len.push(y.len() as u32);
+                }
+                b
+            }
+            fn c_pairs(&self) -> b2a_pairs {
+                b2a_pairs {
+                    seq_blob: self.blob.as_ptr(),
+                    x_off: self.x_off.as_ptr(),
+                    x_len: self.x_len.as_ptr(),
+                    y_off: self.y_off.as_ptr(),
+                    y_len: self.y_len.as_ptr(),
+                    blob_bytes: self.blob.len() as u64,
+                    n_pairs: self.x_len.len() as u64,
+                }
+            }
+        }
+
+        /// Run `f` on this thread's engine; a failing call panics with the engine's error text (no CPU fallback).
+        fn with_engine(f: impl FnOnce(*mut c_void) -> i32) {
+            ENGINE.with(|cell| {
+                let mut eng = cell.borrow_mut();
+                if eng.0.is_null() {
+                    let mut h: *mut c_void = std::ptr::null_mut();
+                    let rc = unsafe { b2a_engine_create(&mut h, 0) };
+                    assert!(rc == 0, "b200align: cannot create an engine on device 0 (rc = {})", rc);
+                    eng.0 = h;
+                }
+                let rc = f(eng.0);
+                if rc != 0 {
+                    let msg = unsafe { CStr::from_ptr(b2a_last_error(eng.0)) }.to_string_lossy().into_owned();
+                    panic!("b200align: {} (rc = {})", msg, rc);
+                }
+            })
+        }
+
+        fn levenshtein_k(pairs: &[(&[u8], &[u8])], k: u32) -> Vec<u32> {
+            let mut out = vec![0u32; pairs.len()];
+            if pairs.is_empty() {
+                return out;
+            }
+            let b = Batch::new(pairs);
+            let cp = b.c_pairs();
+            with_engine(|e| unsafe { b2a_levenshtein_batch(e, k, &cp, out.as_mut_ptr(), std::ptr::null_mut()) });
+            out
+        }
+
+        /// Hamming distances of pairs already checked to have equal lengths
+        fn hamming_equal(pairs: &[(&[u8], &[u8])]) -> Vec<u64> {
+            let mut out = vec![0u32; pairs.len()];
+            let mut status = vec![PAIR_OK; pairs.len()];
+            if !pairs.is_empty() {
+                let b = Batch::new(pairs);
+                let cp = b.c_pairs();
+                with_engine(|e| unsafe { b2a_hamming_batch(e, &cp, out.as_mut_ptr(), status.as_mut_ptr(), std::ptr::null_mut()) });
+            }
+            out.into_iter().map(u64::from).collect()
+        }
+
+        /// distance.rs:25-40; panics with the reference's message on unequal lengths (a batch: on the first such pair)
+        pub fn hamming_batch(pairs: &[(&[u8], &[u8])]) -> Vec<u64> {
+            for (x, y) in pairs {
+                assert_eq!(x.len(), y.len(), "hamming distance cannot be calculated for texts of different length ({}!={})",
+                           x.len(), y.len());
+            }
+            hamming_equal(pairs)
+        }
+
+        /// levenshtein over a batch (distance.rs:59-61)
+        pub fn levenshtein_batch(pairs: &[(&[u8], &[u8])]) -> Vec<u32> {
+            levenshtein_k(pairs, DIST_NONE)
+        }
+
+        pub fn hamming(alpha: &[u8], beta: &[u8]) -> u64 {
+            hamming_batch(&[(alpha, beta)])[0]
+        }
+
+        pub fn levenshtein(alpha: &[u8], beta: &[u8]) -> u32 {
+            levenshtein_batch(&[(alpha, beta)])[0]
+        }
+
+        /// distance.rs:63-173: the same values as the scalar functions
+        pub mod simd {
+            /// distance.rs:101-111, with simd::hamming's own panic message
+            pub fn hamming_batch(pairs: &[(&[u8], &[u8])]) -> Vec<u64> {
+                for (x, y) in pairs {
+                    assert_eq!(x.len(), y.len(),
+                               "simd hamming distance cannot be calculated for texts of different length ({}!={})",
+                               x.len(), y.len());
+                }
+                super::hamming_equal(pairs)
+            }
+
+            pub fn levenshtein_batch(pairs: &[(&[u8], &[u8])]) -> Vec<u32> {
+                super::levenshtein_batch(pairs)
+            }
+
+            /// distance.rs:165-172: per pair the distance if it is <= min(k, max(|x|, |y|)), else None
+            pub fn bounded_levenshtein_batch(pairs: &[(&[u8], &[u8])], k: u32) -> Vec<Option<u32>> {
+                let d = super::levenshtein_k(pairs, k);
+                if k == super::DIST_NONE {
+                    return d.into_iter().map(Some).collect();  // u32::MAX bounds nothing: every distance is Some
+                }
+                d.into_iter().map(|v| if v == super::DIST_NONE { None } else { Some(v) }).collect()
+            }
+
+            pub fn hamming(alpha: &[u8], beta: &[u8]) -> u64 {
+                hamming_batch(&[(alpha, beta)])[0]
+            }
+
+            pub fn levenshtein(alpha: &[u8], beta: &[u8]) -> u32 {
+                levenshtein_batch(&[(alpha, beta)])[0]
+            }
+
+            pub fn bounded_levenshtein(alpha: &[u8], beta: &[u8], k: u32) -> Option<u32> {
+                bounded_levenshtein_batch(&[(alpha, beta)], k)[0]
             }
         }
     }
