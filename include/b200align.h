@@ -430,6 +430,45 @@ int32_t b2a_multi_levenshtein_batch(b2a_multi* m, uint32_t k, const b2a_pairs* p
 int32_t b2a_multi_hamming_batch(b2a_multi* m, const b2a_pairs* pairs, uint32_t* distance, uint32_t* status,
                                 b2a_stats* stats);
 
+/* ---- bio::pattern_matching::myers (reference src/pattern_matching/myers) over a batch of (pattern x, text y) pairs.
+ * The pattern is always x, also when it is longer than the text.  D[i][j] is the unit-cost edit distance with
+ * D[0][j] = 0 (the text is free at both ends) and D[i][0] = i; pattern byte p matches text byte t when t == p, when
+ * bit t of match->ambig row p is set (MyersBuilder::ambig: the pattern side only), or when t is a text wildcard
+ * (MyersBuilder::text_wildcard).  match may be NULL, and either table in it.  Per pair:
+ *   best_end[p], best_dist[p]: find_best_end, the FIRST end j - 1 (0-based) of the least D[m][j], and that distance
+ *     (Myers::distance).  An empty text gives B2A_DIST_NONE for both.
+ *   with n_hits set (a listing), every (j - 1, D[m][j]) with D[m][j] <= k, j = 1..n, in ascending end order
+ *     (find_all_end); *n_hits = their total over the batch.  The hits stay on the engine until its next call of any
+ *     kind and are copied out by b2a_myers_hits_fetch.  A listing whose hits (8 bytes each) are above the engine's
+ *     device-memory budget (b2a_engine_set_traceback_budget; by default 60 % of the free memory) is refused with
+ *     B2A_E_CAPACITY before the hits are allocated.  n_hits NULL: k is ignored and nothing is held.
+ * An empty pattern (the reference panics: "Pattern is empty") is B2A_PAIR_PANIC in `status`, with best_end =
+ * best_dist = B2A_DIST_NONE and no hits; without a status array it fails the call with B2A_E_INVALID naming the pair.
+ * Myers/Hyyro bit-parallel columns over the batch's compacted alphabet: a thread with the pattern in registers up to
+ * 256 symbols, a warp on 2048-row strips beyond.  Several pairs may share one x offset (one pattern, many texts).
+ * stats: cells = sum of m * n, pack_ms = the blob's rewrite into alphabet codes, fill_ms = pass 1 (best ends and hit
+ * counts), walk_ms = the listing's offsets and pass 2 (the pairs with hits rerun to write them), kernel_launches. */
+typedef struct b2a_myers_match {
+  const uint8_t* ambig;     /* NULL, or 256 rows x 32 bytes: bit t of row p = pattern byte p also matches text byte t */
+  const uint8_t* wildcards; /* NULL, or 32 bytes: bit t = text byte t is matched by every pattern byte */
+} b2a_myers_match;
+int32_t b2a_myers_batch(b2a_engine* e, const b2a_myers_match* match, uint32_t k, const b2a_pairs* pairs,
+                        uint32_t* best_end, uint32_t* best_dist, uint64_t* n_hits, uint32_t* status, b2a_stats* stats);
+/* The held listing: hit_off[0..n_pairs] (pair p's hits are [hit_off[p], hit_off[p + 1])), hit_end and hit_dist of
+ * *n_hits entries each.  B2A_E_STATE unless the engine's last call was b2a_myers_batch with a listing. */
+int32_t b2a_myers_hits_fetch(b2a_engine* e, uint64_t* hit_off, uint32_t* hit_end, uint32_t* hit_dist);
+/* How the pairs of the last b2a_myers_batch ran (a measurement aid; results do not depend on it): counts[0] answered
+ * on the host (an empty side), counts[1..4] a thread with the pattern's 1..4 words in registers, counts[5] a warp,
+ * counts[6] the pairs with hits that pass 2 reran.  Up to n_counts (at most 7) entries are written. */
+int32_t b2a_myers_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts);
+/* The multi forms split the pair list as b2a_multi_levenshtein_batch does: each device writes its share of best_end,
+ * best_dist (and status) at its offset, and *n_hits is the sum.  The fetch places each device's hits at its offset
+ * with hit_off rebased; B2A_E_STATE unless the last b2a_multi_* call was b2a_multi_myers_batch with a listing. */
+int32_t b2a_multi_myers_batch(b2a_multi* m, const b2a_myers_match* match, uint32_t k, const b2a_pairs* pairs,
+                              uint32_t* best_end, uint32_t* best_dist, uint64_t* n_hits, uint32_t* status,
+                              b2a_stats* stats);
+int32_t b2a_multi_myers_hits_fetch(b2a_multi* m, uint64_t* hit_off, uint32_t* hit_end, uint32_t* hit_dist);
+
 /* Measurement utility for the int32-ALU roofline (SURVEY 8d): tera lane-ops/s of
  * independent add / min-max / add+max register chains over all SMs of the device. */
 int32_t b2a_util_int32_peak(int32_t device_id, float* tops_add, float* tops_minmax, float* tops_mixed);

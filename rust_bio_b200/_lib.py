@@ -35,6 +35,7 @@ ABI_SYMBOLS = [
     "b2a_multi_exchange_kind", "b2a_multi_align_batch", "b2a_multi_align_batch_banded", "b2a_multi_align_batch_scores",
     "b2a_multi_align_batch_banded_scores",
     "b2a_levenshtein_batch", "b2a_hamming_batch", "b2a_distance_tier_pairs", "b2a_multi_levenshtein_batch", "b2a_multi_hamming_batch",
+    "b2a_myers_batch", "b2a_myers_hits_fetch", "b2a_myers_tier_pairs", "b2a_multi_myers_batch", "b2a_multi_myers_hits_fetch",
     "b2a_util_int32_peak",
 ]
 
@@ -64,6 +65,11 @@ class CBandHints(C.Structure):
     """b2a_band_hints (include/b200align.h)"""
     _fields_ = [("match_off", C.c_void_p), ("match_xy", C.c_void_p), ("path_off", C.c_void_p),
                 ("path_idx", C.c_void_p), ("allowed_mismatches", C.c_int32), ("use_lcskpp_union", C.c_int32)]
+
+
+class CMyersMatch(C.Structure):
+    """b2a_myers_match (include/b200align.h): 256 x 32-byte ambiguity rows and a 32-byte wildcard set, each or NULL"""
+    _fields_ = [("ambig", C.c_void_p), ("wildcards", C.c_void_p)]
 
 
 class CResults(C.Structure):
@@ -174,6 +180,12 @@ def load():
     L.b2a_distance_tier_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.b2a_multi_levenshtein_batch.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(CPairs), C.c_void_p, C.POINTER(CStats)]
     L.b2a_multi_hamming_batch.argtypes = [C.c_void_p, C.POINTER(CPairs), C.c_void_p, C.c_void_p, C.POINTER(CStats)]
+    for pre in ("b2a_", "b2a_multi_"):
+        getattr(L, pre + "myers_batch").argtypes = [C.c_void_p, C.POINTER(CMyersMatch), C.c_uint32, C.POINTER(CPairs),
+                                                    C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p,
+                                                    C.POINTER(CStats)]
+        getattr(L, pre + "myers_hits_fetch").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.b2a_myers_tier_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.b2a_util_int32_peak.argtypes = [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                       C.POINTER(C.c_float)]
     for name in ABI_SYMBOLS:

@@ -74,8 +74,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
     eo = os.path.join(OBJ, "engine.o")
     objs.append(eo)
     esrc = os.path.join(CSRC, "b2a_engine.cu")
-    dist_h = os.path.join(CSRC, "b2a_distance.cuh")  # engine.o and distance.o only
-    if force or _stale(eo, hdrs + [esrc, dist_h]):
+    dist_h = os.path.join(CSRC, "b2a_distance.cuh")  # engine.o, distance.o and myers.o only
+    myers_h = os.path.join(CSRC, "b2a_myers.cuh")  # engine.o and myers.o only
+    if force or _stale(eo, hdrs + [esrc, dist_h, myers_h]):
         jobs.append([NVCC, *FLAGS, "-c", esrc, "-o", eo])
     so = os.path.join(OBJ, "banded_strip_notb.o")  # the strip fill's score-only twins, beside engine.o
     objs.append(so)
@@ -87,6 +88,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
     dsrc = os.path.join(CSRC, "b2a_distance.cu")
     if force or _stale(do, hdrs + [dsrc, dist_h]):
         jobs.append([NVCC, *FLAGS, "-c", dsrc, "-o", do])
+    yo = os.path.join(OBJ, "myers.o")  # the pattern-matching kernels (b2a_myers.cuh: their lane logic)
+    objs.append(yo)
+    ysrc = os.path.join(CSRC, "b2a_myers.cu")
+    if force or _stale(yo, hdrs + [ysrc, dist_h, myers_h]):
+        jobs.append([NVCC, *FLAGS, "-c", ysrc, "-o", yo])
     mo = os.path.join(OBJ, "multi.o")
     objs.append(mo)
     msrc = os.path.join(CSRC, "b2a_multi.cu")

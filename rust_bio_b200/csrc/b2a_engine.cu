@@ -24,6 +24,7 @@
 #include "b2a_banded.cuh"
 #include "b2a_banded_strip.cuh"
 #include "b2a_distance.cuh"
+#include "b2a_myers.cuh"
 
 using namespace b2a;
 
@@ -121,6 +122,10 @@ struct b2a_engine {
   bool banded_strip_lastcol = true;  // ... also for bands reaching column n (B2A_BANDED_STRIP_LASTCOL=0: those stay with K3)
   uint64_t strip_pairs = 0;  // pairs the strip path finished in the last banded call (the rest ran the K3 loops)
   uint64_t dist_tier_pairs[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // pairs per tier of the last b2a_levenshtein_batch (DT_*)
+  // the last b2a_myers_batch: pairs per tier (MT_*) and, last, the pairs pass 2 reran
+  uint64_t myers_tier_pairs[MT_COUNT + 1] = {0, 0, 0, 0, 0, 0, 0};
+  bool myers_held = false;  // its hit list (d_hoff, d_hend, d_hdist) stays on the device until the next call
+  uint64_t myers_hits = 0;
   // packed input (b2a_align_batch_packed): the caller's "blob" is BitEnc storage of this width (0 = bytes); the
   // engine unpacks it on the device and uses its own byte offsets (eff_xoff / eff_yoff) from then on
   uint32_t packed_width = 0;
@@ -154,7 +159,8 @@ struct b2a_engine {
       d_rowm, d_fin, d_tb, d_opsscratch, d_lut, d_codemap, d_ctl, d_score, d_xs, d_xe, d_ys, d_ye, d_nops,
       d_opssrc, d_clip, d_status, d_nops64, d_opsoff, d_opsdense, d_scan, d_records, d_prog, d_bcells, d_bstatus,
       d_bopsend, d_bslab, d_branges, d_broff, d_bfill, d_bfoff, d_hmoff, d_hmxy, d_hpoff, d_hpidx, d_raw, d_gnops,
-      d_gnops64, d_goff, d_bcols, d_bstrip, d_bsoff, d_belig, d_ckpt, d_rcbnd, d_rcstate;
+      d_gnops64, d_goff, d_bcols, d_bstrip, d_bsoff, d_belig, d_ckpt, d_rcbnd, d_rcstate, d_mmatch, d_hoff, d_hend,
+      d_hdist;
   uint32_t* h_nops = nullptr;  // pinned staging of b2a_gathered_fetch
   uint64_t h_nops_cap = 0;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -345,7 +351,7 @@ int32_t b2a_engine_destroy(b2a_engine* e) {
                     &e->d_bstatus, &e->d_bopsend, &e->d_bslab, &e->d_branges, &e->d_broff, &e->d_bfill, &e->d_hmoff, &e->d_hmxy,
                     &e->d_hpoff, &e->d_hpidx, &e->d_raw, &e->d_gnops, &e->d_gnops64, &e->d_goff,
                     &e->d_bfoff, &e->d_bcols, &e->d_bstrip, &e->d_bsoff, &e->d_belig, &e->d_ckpt, &e->d_rcbnd,
-                    &e->d_rcstate};
+                    &e->d_rcstate, &e->d_mmatch, &e->d_hoff, &e->d_hend, &e->d_hdist};
   for (DevBuf* b : bufs) b->release();
   for (auto& v : e->ev)
     if (v) cudaEventDestroy(v);
@@ -459,7 +465,7 @@ static void compact_codemap(b2a_engine* e, const std::vector<int>& syms) {
 static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, const b2a_pairs* pairs,
                            uint32_t& maxm, uint32_t& maxn, int64_t& score_bound) {
   if (!e || !s || !pairs) return B2A_E_INVALID;
-  e->staged = e->ran = e->banded_held = false;
+  e->staged = e->ran = e->banded_held = e->myers_held = false;
   e->score_only = false;
   e->rc_waves.clear();
   e->rc_pairs = e->rc_windows = e->rc_filled = 0;
@@ -614,6 +620,19 @@ static int32_t stage_front(b2a_engine* e, int32_t mode, const b2a_scoring* s, co
 // the finish region of a launch whose blocks start `lo` blocks into the wave (F_FINISH; null stays null)
 static int32_t* fin_from(int32_t* fin, uint32_t lo) { return fin ? fin + (size_t)lo * FIN_FIELDS * 32 : nullptr; }
 
+// n + 1 offsets of n u32 counts (the exclusive sum and the total): widen to u64 with a trailing 0 (into `wide`,
+// n + 1 words), then a device-wide scan (three launches in all)
+static int32_t scan_offsets(b2a_engine* e, const uint32_t* cnt, uint64_t* wide, uint64_t* off, uint64_t n,
+                            cudaStream_t st) {
+  widen_kernel<<<(unsigned)((n + 1 + 255) / 256), 256, 0, st>>>(cnt, wide, n);
+  CK(cudaGetLastError());
+  size_t tmp = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, wide, off, (int64_t)(n + 1), st));
+  CK(e->d_scan.reserve(tmp + 16));
+  CK(cub::DeviceScan::ExclusiveSum(e->d_scan.p, tmp, wide, off, (int64_t)(n + 1), st));
+  return B2A_OK;
+}
+
 // ops compaction shared by the full and the banded path: widen -> exclusive scan -> gather
 static int32_t compact_ops(b2a_engine* e, uint64_t scratch_bytes, cudaStream_t st) {
   const uint64_t n = e->n_pairs;
@@ -622,15 +641,9 @@ static int32_t compact_ops(b2a_engine* e, uint64_t scratch_bytes, cudaStream_t s
       scan_small_kernel<<<1, 1024, 0, st>>>(e->d_nops.as<uint32_t>(), e->d_opsoff.as<uint64_t>(), (uint32_t)n);
       CK(cudaGetLastError());
     } else {
-    const unsigned g1 = (unsigned)((n + 1 + 255) / 256);
-    widen_kernel<<<g1, 256, 0, st>>>(e->d_nops.as<uint32_t>(), e->d_nops64.as<uint64_t>(), n);
-    CK(cudaGetLastError());
-    size_t tmp = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp, e->d_nops64.as<uint64_t>(), e->d_opsoff.as<uint64_t>(),
-                                     (int64_t)(n + 1), st));
-    CK(e->d_scan.reserve(tmp + 16));
-    CK(cub::DeviceScan::ExclusiveSum(e->d_scan.p, tmp, e->d_nops64.as<uint64_t>(),
-                                     e->d_opsoff.as<uint64_t>(), (int64_t)(n + 1), st));
+      const int32_t rc = scan_offsets(e, e->d_nops.as<uint32_t>(), e->d_nops64.as<uint64_t>(),
+                                      e->d_opsoff.as<uint64_t>(), n, st);
+      if (rc) return rc;
     }
     // worst case every pair emits m+n+4 ops; size the dense buffer by the scratch size
     CK(e->d_opsdense.reserve(scratch_bytes + 16));
@@ -1585,7 +1598,7 @@ int32_t b2a_align_batch(b2a_engine* e, int32_t mode, const b2a_scoring* scoring,
   if (!e || !scoring || !pairs) return B2A_E_INVALID;
   // large batches with host outputs: pipeline chunks so copies and planning overlap the kernels
   if (e->pipe_chunks >= 2 && results && pairs->n_pairs >= 262144) {
-    e->staged = e->ran = e->banded_held = false;
+    e->staged = e->ran = e->banded_held = e->myers_held = false;
     e->score_only = false;
     e->rc_pairs = e->rc_windows = e->rc_filled = 0;
     if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
@@ -2378,7 +2391,7 @@ int32_t b2a_records_decode(const void* host_records, uint32_t stride, uint64_t n
 // What the distance calls share before any device work: the engine's staged state is dropped (they reuse its
 // buffers), the pair count and every offset + length are checked against the blob, and the pair arrays are uploaded.
 static int32_t dist_front(b2a_engine* e, const b2a_pairs* pairs) {
-  e->staged = e->ran = e->banded_held = false;
+  e->staged = e->ran = e->banded_held = e->myers_held = false;
   e->score_only = false;
   if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
   const uint64_t n = pairs->n_pairs;
@@ -2559,6 +2572,253 @@ int32_t b2a_hamming_batch(b2a_engine* e, const b2a_pairs* pairs, uint32_t* dista
   }
   CK(cudaEventRecord(e->ev[2], st));
   return dist_finish(e, distance, done, cells, true, stats);
+}
+
+}  // extern "C"
+
+// ---- batched Myers pattern matching (bio::pattern_matching::myers): kernels and lane logic in b2a_myers.cu / .cuh
+
+// The call's ambiguity rows and wildcard set as a relation over the batch's codes, uploaded to d_mmatch as
+// [rel_off: sigma + 1 words][wild: 256 codes][rel: codes]: pattern code a also matches rel[rel_off[a]..rel_off[a+1]),
+// every wild code matches every pattern code.  Bytes absent from the blob have no code and drop out; with nothing
+// left the masks are built by the identity loop (rel_off == nullptr).
+static int32_t myers_relation(b2a_engine* e, const b2a_myers_match* match, const std::vector<int>& syms,
+                              MyersMatch* out) {
+  *out = MyersMatch{nullptr, nullptr, nullptr, 0};
+  if (!match || (!match->ambig && !match->wildcards)) return B2A_OK;
+  const int sigma = (int)syms.size();
+  auto bit = [](const uint8_t* row, int t) { return (row[t >> 3] >> (t & 7)) & 1; };
+  std::vector<uint32_t> off(sigma + 1, 0);
+  std::vector<uint8_t> rel, wild;
+  for (int a = 0; a < sigma; ++a) {
+    off[a] = (uint32_t)rel.size();
+    if (match->ambig)
+      for (int b = 0; b < sigma; ++b)
+        if (b != a && bit(match->ambig + 32 * syms[a], syms[b])) rel.push_back((uint8_t)b);
+  }
+  off[sigma] = (uint32_t)rel.size();
+  if (match->wildcards)
+    for (int b = 0; b < sigma; ++b)
+      if (bit(match->wildcards, syms[b])) wild.push_back((uint8_t)b);
+  if (rel.empty() && wild.empty()) return B2A_OK;
+  const size_t off_bytes = off.size() * 4, bytes = off_bytes + 256 + rel.size();
+  std::vector<uint8_t> h(bytes, 0);
+  std::memcpy(h.data(), off.data(), off_bytes);
+  std::memcpy(h.data() + off_bytes, wild.data(), wild.size());
+  std::memcpy(h.data() + off_bytes + 256, rel.data(), rel.size());
+  CK(e->d_mmatch.reserve(bytes + 16));
+  CK(cudaMemcpyAsync(e->d_mmatch.p, h.data(), bytes, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaStreamSynchronize(e->stream));  // (h is a stack vector)
+  e->h2d_bytes += bytes;
+  const uint8_t* d = e->d_mmatch.as<uint8_t>();
+  *out = MyersMatch{reinterpret_cast<const uint32_t*>(d), d + off_bytes + 256, d + off_bytes, (int)wild.size()};
+  return B2A_OK;
+}
+
+// the tier kernels of one pass: tier t's n_tasks[t] tasks at order + seg.at[t]
+static int32_t myers_pass(b2a_engine* e, MyersArgs a, const uint32_t* order, const MyersSegs& seg,
+                          const uint32_t* n_tasks, int ctas, int wpc, uint64_t bnd_words, uint32_t* ctr) {
+  for (int t = MT_REGS1; t < MT_COUNT; ++t) {
+    a.tasks = order + seg.at[t];
+    a.n_tasks = n_tasks[t];
+    if (!a.n_tasks) continue;
+    if (t == MT_WARP)
+      CK(launch_myers_warp(a, ctas, wpc, e->d_bnd.as<uint32_t>(), bnd_words, ctr, e->stream));
+    else
+      CK(launch_myers_thread(t, a, e->stream));
+    ++e->launches;
+  }
+  return B2A_OK;
+}
+
+extern "C" {
+
+int32_t b2a_myers_batch(b2a_engine* e, const b2a_myers_match* match, uint32_t k, const b2a_pairs* pairs,
+                        uint32_t* best_end, uint32_t* best_dist, uint64_t* n_hits, uint32_t* status,
+                        b2a_stats* stats) {
+  if (!e || !pairs || ((!best_end || !best_dist) && pairs->n_pairs)) return B2A_E_INVALID;
+  int32_t rc = dist_front(e, pairs);  // (a refused batch leaves status untouched)
+  if (rc) return rc;
+  const uint64_t n = pairs->n_pairs;
+  const bool listing = n_hits != nullptr;
+  // an empty pattern: the reference panics (simple.rs / long.rs: "Pattern is empty"); only that pair with a status
+  // array.  The tier of every other pair from its pattern length; tasks grouped by tier, results land by pair index.
+  std::vector<uint32_t> tasks[MT_COUNT];
+  std::vector<std::pair<uint64_t, uint32_t>> done;
+  uint64_t cells = 0;
+  uint32_t warp_maxn = 0;
+  for (uint64_t p = 0; p < n; ++p) {
+    const uint32_t m = pairs->x_len[p], nn = pairs->y_len[p];
+    if (m == 0 && !status) return e->fail(B2A_E_INVALID, "pair " + std::to_string(p) + ": Pattern is empty");
+    cells += (uint64_t)m * nn;
+    const int t = myers_tier(m, nn);
+    if (t == MT_DONE) {
+      done.push_back({p, DIST_NONE});
+      continue;
+    }
+    tasks[t].push_back((uint32_t)p);
+    if (t == MT_WARP) warp_maxn = std::max(warp_maxn, nn);
+  }
+  if (status)
+    for (uint64_t p = 0; p < n; ++p) status[p] = pairs->x_len[p] == 0 ? B2A_PAIR_PANIC : B2A_PAIR_OK;
+  const uint64_t n_dp = n - done.size();
+  e->myers_tier_pairs[MT_DONE] = done.size();
+  for (int t = 1; t < MT_COUNT; ++t) e->myers_tier_pairs[t] = tasks[t].size();
+  e->myers_tier_pairs[MT_COUNT] = 0;
+  cudaStream_t st = e->stream;
+  CK(e->d_xs.reserve(n * 4 + 4));  // best ends (best distances: d_score)
+  CK(e->d_nops.reserve(n * 4 + 4));  // hit counts
+  CK(e->d_ctl.reserve(2048));
+  uint32_t* ctl = e->d_ctl.as<uint32_t>();  // [0] pass 1's warp counter, [1] pass 2's, [2..] pass 2's tier sizes
+  CK(cudaMemsetAsync(ctl, 0, 64, st));
+  if (listing) {
+    CK(e->d_nops64.reserve(n * 8 + 8));
+    CK(e->d_hoff.reserve(n * 8 + 8));
+    if (n) CK(cudaMemsetAsync(e->d_nops.p, 0, n * 4, st));  // the host-answered pairs have no hits
+  }
+  MyersSegs seg{};
+  std::vector<uint32_t> all;
+  int ctas = 0, wpc = 0;
+  const uint64_t bnd_words = ((uint64_t)warp_maxn + 15) / 16;
+  MyersArgs a{};
+  if (n_dp) {
+    // the blob as codes of the batch's alphabet: the match masks are sigma words per pattern word
+    bool present[256];
+    rc = upload_blob(e, pairs, present);
+    if (rc) return rc;
+    const std::vector<int> syms = batch_symbols(e, present);
+    compact_codemap(e, syms);
+    CK(e->d_codemap.reserve(256));
+    CK(cudaMemcpyAsync(e->d_codemap.p, e->codemap_host, 256, cudaMemcpyHostToDevice, st));
+    rc = myers_relation(e, match, syms, &a.match);
+    if (rc) return rc;
+    all.reserve(n_dp);
+    for (int t = MT_REGS1; t < MT_COUNT; ++t) {
+      seg.at[t] = (uint32_t)all.size();
+      all.insert(all.end(), tasks[t].begin(), tasks[t].end());
+    }
+    seg.at[MT_COUNT] = (uint32_t)all.size();
+    CK(e->d_order.reserve(all.size() * 8 + 8));  // pass 1's task lists, then pass 2's
+    CK(cudaMemcpyAsync(e->d_order.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice, st));
+    e->h2d_bytes += 256 + all.size() * 4;
+    const int sigma = (int)syms.size();
+    if (!tasks[MT_WARP].empty()) {
+      CK(myers_warp_grid(sigma, e->num_sms, (uint32_t)tasks[MT_WARP].size(), &ctas, &wpc));
+      CK(e->d_bnd.reserve((uint64_t)ctas * wpc * bnd_words * 4 + 16));
+    }
+    CK(cudaEventRecord(e->ev[0], st));
+    CK(launch_dist_translate(e->d_blob.as<uint8_t>(), pairs->blob_bytes, e->d_codemap.as<uint8_t>(), e->num_sms, st));
+    ++e->launches;
+    CK(cudaEventRecord(e->ev[1], st));
+    a.codes = e->d_blob.as<uint8_t>();
+    a.x_off = e->d_xoff.as<uint64_t>();
+    a.x_len = e->d_xlen.as<uint32_t>();
+    a.y_off = e->d_yoff.as<uint64_t>();
+    a.y_len = e->d_ylen.as<uint32_t>();
+    a.k = k;
+    a.sigma = sigma;
+    a.best_end = e->d_xs.as<uint32_t>();
+    a.best_dist = e->d_score.as<uint32_t>();
+    a.count = listing ? e->d_nops.as<uint32_t>() : nullptr;
+    uint32_t n1[MT_COUNT] = {0};
+    for (int t = MT_REGS1; t < MT_COUNT; ++t) n1[t] = seg.at[t + 1] - seg.at[t];
+    rc = myers_pass(e, a, e->d_order.as<uint32_t>(), seg, n1, ctas, wpc, bnd_words, ctl);
+    if (rc) return rc;
+  } else {
+    CK(cudaEventRecord(e->ev[0], st));
+    CK(cudaEventRecord(e->ev[1], st));
+  }
+  CK(cudaEventRecord(e->ev[2], st));
+  uint64_t total = 0;
+  if (listing) {
+    // pass 2: the offsets of every pair's hits, the pairs with hits per tier, and only those rerun to write them
+    rc = scan_offsets(e, e->d_nops.as<uint32_t>(), e->d_nops64.as<uint64_t>(), e->d_hoff.as<uint64_t>(), n, st);
+    if (rc) return rc;
+    e->launches += 3;
+    uint32_t* order2 = e->d_order.as<uint32_t>() + all.size();
+    if (n_dp) {
+      CK(launch_myers_select(e->d_order.as<uint32_t>(), seg, e->d_nops.as<uint32_t>(), order2, ctl + 2, st));
+      ++e->launches;
+    }
+    CK(cudaEventRecord(e->ev[3], st));
+    uint32_t h_ctl[2 + MT_COUNT];
+    CK(cudaMemcpyAsync(&total, e->d_hoff.as<uint64_t>() + n, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h_ctl, ctl, sizeof(h_ctl), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    uint64_t budget = e->tb_budget;
+    if (!budget) {
+      size_t fr = 0, tot = 0;
+      CK(cudaMemGetInfo(&fr, &tot));
+      budget = (uint64_t)((double)fr * 0.6);
+    }
+    if (total > budget / 8)
+      return e->fail(B2A_E_CAPACITY, "the listing holds " + std::to_string(total) + " hits (" +
+                                          std::to_string(total * 8) + " bytes), above the device-memory budget of " +
+                                          std::to_string(budget) + " bytes");
+    CK(e->d_hend.reserve(total * 4 + 16));
+    CK(e->d_hdist.reserve(total * 4 + 16));
+    uint64_t rerun = 0;
+    for (int t = MT_REGS1; t < MT_COUNT; ++t) rerun += h_ctl[2 + t];
+    e->myers_tier_pairs[MT_COUNT] = rerun;
+    CK(cudaEventRecord(e->ev[4], st));
+    if (rerun) {  // the same segments of the second list, each holding its first h_ctl[2 + t] tasks
+      a.hit_off = e->d_hoff.as<uint64_t>();
+      a.hit_end = e->d_hend.as<uint32_t>();
+      a.hit_dist = e->d_hdist.as<uint32_t>();
+      rc = myers_pass(e, a, order2, seg, h_ctl + 2, ctas, wpc, bnd_words, ctl + 1);
+      if (rc) return rc;
+    }
+    CK(cudaEventRecord(e->ev[5], st));
+  }
+  if (n) {
+    CK(cudaMemcpyAsync(best_end, e->d_xs.p, n * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(best_dist, e->d_score.p, n * 4, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  for (const auto& pv : done) best_end[pv.first] = best_dist[pv.first] = pv.second;
+  if (listing) {
+    *n_hits = total;
+    e->myers_hits = total;
+    e->myers_held = true;
+  }
+  if (stats) {
+    std::memset(stats, 0, sizeof(*stats));
+    stats->cells = cells;
+    stats->h2d_bytes = e->h2d_bytes;
+    stats->d2h_bytes = n * 8 + (listing ? 8 : 0);
+    cudaEventElapsedTime(&stats->pack_ms, e->ev[0], e->ev[1]);
+    cudaEventElapsedTime(&stats->fill_ms, e->ev[1], e->ev[2]);
+    if (listing) {
+      float scan_ms = 0, pass2_ms = 0;
+      cudaEventElapsedTime(&scan_ms, e->ev[2], e->ev[3]);
+      cudaEventElapsedTime(&pass2_ms, e->ev[4], e->ev[5]);
+      stats->walk_ms = scan_ms + pass2_ms;
+    }
+    stats->kernel_launches = e->launches;
+  }
+  return B2A_OK;
+}
+
+int32_t b2a_myers_hits_fetch(b2a_engine* e, uint64_t* hit_off, uint32_t* hit_end, uint32_t* hit_dist) {
+  if (!e) return B2A_E_INVALID;
+  if (!e->myers_held)
+    return e->fail(B2A_E_STATE, "no hits are held: the engine's last call was not b2a_myers_batch with a listing");
+  if (!hit_off || ((!hit_end || !hit_dist) && e->myers_hits)) return B2A_E_INVALID;
+  if (cudaSetDevice(e->device) != cudaSuccess) return e->fail(B2A_E_NO_DEVICE, "cudaSetDevice failed");
+  cudaStream_t st = e->stream;
+  CK(cudaMemcpyAsync(hit_off, e->d_hoff.p, (e->n_pairs + 1) * 8, cudaMemcpyDeviceToHost, st));
+  if (e->myers_hits) {
+    CK(cudaMemcpyAsync(hit_end, e->d_hend.p, e->myers_hits * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(hit_dist, e->d_hdist.p, e->myers_hits * 4, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  return B2A_OK;
+}
+
+int32_t b2a_myers_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts) {
+  if (!e || (!counts && n_counts)) return B2A_E_INVALID;
+  for (uint32_t t = 0; t < n_counts && t <= (uint32_t)MT_COUNT; ++t) counts[t] = e->myers_tier_pairs[t];
+  return B2A_OK;
 }
 
 }  // extern "C"

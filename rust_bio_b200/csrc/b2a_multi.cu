@@ -54,6 +54,13 @@ struct b2a_multi {
   std::vector<nccl_comm_t> comms;
   bool use_nccl = false;
   bool repeated = false;  // a device is listed more than once: one engine per entry, peer copies onto entry 0
+  // the engines holding the last call's Myers hit list (b2a_multi_myers_batch with a listing; empty after any other
+  // call): entry d's pairs [lo, hi) of the caller's list and its hit count, in pair order
+  struct HeldHits {
+    size_t d;
+    uint64_t lo, hi, hits;
+  };
+  std::vector<HeldHits> myers_held;
   std::string err;
   int fail(int code, const std::string& what) {
     err = what;
@@ -215,6 +222,7 @@ int32_t run_split(b2a_multi* m, const b2a_pairs* pairs, b2a_results* results, b2
                   const WholeJob& whole, const ShareJob& job) {
   const size_t nd = m->devs.size();
   const uint64_t n = pairs->n_pairs;
+  m->myers_held.clear();
   if (nd == 1 || n < nd) {
     cudaSetDevice(m->devs[0]);
     const int rc = whole(m->eng[0]);
@@ -500,6 +508,73 @@ int32_t b2a_multi_hamming_batch(b2a_multi* m, const b2a_pairs* pairs, uint32_t* 
       [&](b2a_engine* e, const Share& s, b2a_stats* st) {
         return b2a_hamming_batch(e, &s.pairs, distance + s.lo, status ? status + s.lo : nullptr, st);
       });
+}
+
+}  // extern "C"
+
+extern "C" {
+
+int32_t b2a_multi_myers_batch(b2a_multi* m, const b2a_myers_match* match, uint32_t k, const b2a_pairs* pairs,
+                              uint32_t* best_end, uint32_t* best_dist, uint64_t* n_hits, uint32_t* status,
+                              b2a_stats* stats) {
+  if (!m || !pairs || ((!best_end || !best_dist) && pairs->n_pairs)) return B2A_E_INVALID;
+  if (!status && m->devs.size() > 1) {
+    // an empty pattern fails the call; a share would name it by its index in the share, so the whole batch is
+    // checked here first (offsets, then patterns, in the single engine's order) and the caller's index reported
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p) {
+      const uint64_t bb = pairs->blob_bytes, xo = pairs->x_off[p], yo = pairs->y_off[p];
+      if (xo > bb || pairs->x_len[p] > bb - xo || yo > bb || pairs->y_len[p] > bb - yo)
+        return m->fail(B2A_E_INVALID, "sequence offset/length outside seq_blob");
+    }
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p)
+      if (pairs->x_len[p] == 0) return m->fail(B2A_E_INVALID, "pair " + std::to_string(p) + ": Pattern is empty");
+  }
+  const size_t nd = m->devs.size();
+  std::vector<uint64_t> hits(nd, 0);
+  std::vector<b2a_multi::HeldHits> held;
+  const int32_t rc = run_split(
+      m, pairs, nullptr, stats, false,
+      [&](b2a_engine* e) {
+        held = {{0, 0, pairs->n_pairs, 0}};
+        return b2a_myers_batch(e, match, k, pairs, best_end, best_dist, n_hits ? &held[0].hits : nullptr, status,
+                               stats);
+      },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        const size_t d = (size_t)(std::find(m->eng.begin(), m->eng.end(), e) - m->eng.begin());
+        return b2a_myers_batch(e, match, k, &s.pairs, best_end + s.lo, best_dist + s.lo, n_hits ? &hits[d] : nullptr,
+                               status ? status + s.lo : nullptr, st);
+      });
+  if (rc || !n_hits) return rc;
+  if (held.empty()) {  // the split ran: every entry holds its share
+    const uint64_t per = (pairs->n_pairs + nd - 1) / nd;
+    for (size_t d = 0; d < nd; ++d) {
+      const uint64_t lo = std::min<uint64_t>(pairs->n_pairs, d * per);
+      held.push_back({d, lo, std::min<uint64_t>(pairs->n_pairs, lo + per), hits[d]});
+    }
+  }
+  *n_hits = 0;
+  for (const auto& h : held) *n_hits += h.hits;
+  m->myers_held = held;
+  return B2A_OK;
+}
+
+int32_t b2a_multi_myers_hits_fetch(b2a_multi* m, uint64_t* hit_off, uint32_t* hit_end, uint32_t* hit_dist) {
+  if (!m) return B2A_E_INVALID;
+  if (m->myers_held.empty())
+    return m->fail(B2A_E_STATE, "no hits are held: the last call was not b2a_multi_myers_batch with a listing");
+  if (!hit_off) return B2A_E_INVALID;
+  // one share after the other: a share's last offset is the next share's first, rewritten by it
+  uint64_t base = 0;
+  for (const auto& h : m->myers_held) {
+    cudaSetDevice(m->devs[h.d]);
+    const int32_t rc = b2a_myers_hits_fetch(m->eng[h.d], hit_off + h.lo, hit_end ? hit_end + base : nullptr,
+                                            hit_dist ? hit_dist + base : nullptr);
+    if (rc) return m->fail(rc, std::string("device ") + std::to_string(m->devs[h.d]) + ": " +
+                                   b2a_last_error(m->eng[h.d]));
+    for (uint64_t p = h.lo; p <= h.hi; ++p) hit_off[p] += base;
+    base += h.hits;
+  }
+  return B2A_OK;
 }
 
 }  // extern "C"

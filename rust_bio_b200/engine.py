@@ -7,7 +7,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 from . import _lib
-from ._lib import B2AError, CPairs, CResults, CScoring, CStats
+from ._lib import B2AError, CMyersMatch, CPairs, CResults, CScoring, CStats
 
 Batch = Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]
 
@@ -87,7 +87,7 @@ class ScoreResults:
 
 class _BatchCalls:
     """The batch methods Engine and MultiEngine share: host arrays in, host results out.  A subclass binds the C entry
-    points (_c_align, _c_scores, _c_banded, _c_banded_scores, _c_levenshtein, _c_hamming: the handle's calls, each returning the rc) and _check."""
+    points (_c_align, _c_scores, _c_banded, _c_banded_scores, _c_levenshtein, _c_hamming, _c_myers, _c_myers_fetch: the handle's calls, each returning the rc) and _check."""
 
     @staticmethod
     def _cpairs(batch: Batch):
@@ -202,6 +202,58 @@ class _BatchCalls:
                                     st.ctypes.data_as(C.c_void_p) if pair_status else None))
         return (out[:n], st[:n]) if pair_status else out[:n]
 
+    def myers_batch(self, batch: Batch, k: Optional[int] = None, ambig=None, wildcards=None,
+                    pair_status: bool = True) -> Dict[str, np.ndarray]:
+        """b2a_myers_batch: per pair, the semi-global search of the pattern x in the text y (bio::pattern_matching::
+        myers) -> {"best_end", "best_dist"} (uint32, DIST_NONE for an empty text or pattern), "status" (B2A_PAIR_*:
+        an empty pattern is B2A_PAIR_PANIC) with pair_status, and with k every end whose distance is <= k as CSR:
+        "hit_off" (uint64, n + 1), "hit_end", "hit_dist" (uint32).  k above u32 is clamped: a distance is at most the
+        pattern length.  ambig: {pattern byte: text bytes it also matches}; wildcards: text bytes every pattern byte
+        matches (MyersBuilder.ambig / text_wildcard).  pair_status=False: an empty pattern fails the call."""
+        if k is not None and int(k) < 0:
+            raise ValueError("k must be >= 0")
+        n = len(batch[2])
+        best_end = np.zeros(max(1, n), dtype=np.uint32)
+        best_dist = np.zeros(max(1, n), dtype=np.uint32)
+        st = np.zeros(max(1, n), dtype=np.uint32) if pair_status else None
+        cm, keep = myers_match(ambig, wildcards)
+        cp = self._cpairs(batch)
+        hits = C.c_uint64(0)
+        p = lambda a: a.ctypes.data_as(C.c_void_p)
+        self._check(self._c_myers(C.byref(cm) if cm is not None else None,
+                                  0 if k is None else min(int(k), _lib.DIST_NONE), C.byref(cp), p(best_end),
+                                  p(best_dist), C.byref(hits) if k is not None else None,
+                                  p(st) if pair_status else None))
+        del keep
+        out = {"best_end": best_end[:n], "best_dist": best_dist[:n]}
+        if pair_status:
+            out["status"] = st[:n]
+        if k is not None:
+            h = int(hits.value)
+            off = np.zeros(n + 1, dtype=np.uint64)
+            he = np.zeros(max(1, h), dtype=np.uint32)
+            hd = np.zeros(max(1, h), dtype=np.uint32)
+            self._check(self._c_myers_fetch(p(off), p(he), p(hd)))
+            out.update(hit_off=off, hit_end=he[:h], hit_dist=hd[:h])
+        return out
+
+
+def myers_match(ambig=None, wildcards=None):
+    """(CMyersMatch or None, the arrays it points to): the bit tables of b2a_myers_match from {pattern byte:
+    equivalent text bytes} and an iterable of wildcard text bytes"""
+    if not ambig and not wildcards:
+        return None, None
+    amb = np.zeros((256, 32), dtype=np.uint8) if ambig else None
+    for p, eqs in (ambig or {}).items():
+        for t in bytes(eqs):
+            amb[int(p), t >> 3] |= np.uint8(1 << (t & 7))
+    wild = np.zeros(32, dtype=np.uint8) if wildcards else None
+    for t in (wildcards or ()):
+        wild[int(t) >> 3] |= np.uint8(1 << (int(t) & 7))
+    cm = CMyersMatch(amb.ctypes.data_as(C.c_void_p) if amb is not None else None,
+                     wild.ctypes.data_as(C.c_void_p) if wild is not None else None)
+    return cm, (amb, wild)
+
 
 class Engine(_BatchCalls):
     def __init__(self, device: int = 0):
@@ -265,6 +317,13 @@ class Engine(_BatchCalls):
         self._check(self._L.b2a_engine_last_recompute(self._h, C.byref(p), C.byref(w), C.byref(f)))
         return {"pairs": int(p.value), "windows": int(w.value), "windows_filled": int(f.value)}
 
+    def myers_tier_pairs(self) -> list:
+        """Pairs of the last myers_batch per tier: [host-answered, register tier with 1..4 words (4 entries), warp,
+        pairs rerun by pass 2 to write their hits] (b2a_myers_tier_pairs; a measurement aid)."""
+        buf = np.zeros(7, dtype=np.uint64)
+        self._check(self._L.b2a_myers_tier_pairs(self._h, buf.ctypes.data_as(C.c_void_p), 7))
+        return [int(v) for v in buf]
+
     def distance_tier_pairs(self) -> list:
         """Pairs of the last levenshtein_batch per tier: [host-answered, register tier with 1..4 words (4 entries),
         4-word band, 8-word band, warp] (b2a_distance_tier_pairs; a measurement aid)."""
@@ -289,6 +348,12 @@ class Engine(_BatchCalls):
 
     def _c_hamming(self, cp, out, status):
         return self._L.b2a_hamming_batch(self._h, cp, out, status, C.byref(self.stats))
+
+    def _c_myers(self, cm, k, cp, best_end, best_dist, n_hits, status):
+        return self._L.b2a_myers_batch(self._h, cm, k, cp, best_end, best_dist, n_hits, status, C.byref(self.stats))
+
+    def _c_myers_fetch(self, off, hit_end, hit_dist):
+        return self._L.b2a_myers_hits_fetch(self._h, off, hit_end, hit_dist)
 
     def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
@@ -482,6 +547,13 @@ class MultiEngine(_BatchCalls):
 
     def _c_hamming(self, cp, out, status):
         return self._L.b2a_multi_hamming_batch(self._h, cp, out, status, C.byref(self.stats))
+
+    def _c_myers(self, cm, k, cp, best_end, best_dist, n_hits, status):
+        return self._L.b2a_multi_myers_batch(self._h, cm, k, cp, best_end, best_dist, n_hits, status,
+                                             C.byref(self.stats))
+
+    def _c_myers_fetch(self, off, hit_end, hit_dist):
+        return self._L.b2a_multi_myers_hits_fetch(self._h, off, hit_end, hit_dist)
 
     def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_multi_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))

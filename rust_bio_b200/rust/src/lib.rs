@@ -875,7 +875,8 @@ pub mod alignment {
         }
 
         /// Run `f` on this thread's engine; a failing call panics with the engine's error text (no CPU fallback).
-        fn with_engine(f: impl FnOnce(*mut c_void) -> i32) {
+        /// `pattern_matching::myers` shares the engine.
+        pub(crate) fn with_engine(f: impl FnOnce(*mut c_void) -> i32) {
             ENGINE.with(|cell| {
                 let mut eng = cell.borrow_mut();
                 if eng.0.is_null() {
@@ -972,6 +973,273 @@ pub mod alignment {
 
             pub fn bounded_levenshtein(alpha: &[u8], beta: &[u8], k: u32) -> Option<u32> {
                 bounded_levenshtein_batch(&[(alpha, beta)], k)[0]
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------- pattern matching, reference src/pattern_matching
+/// `bio::pattern_matching` on the GPU: the Myers bit-parallel search (`myers`).
+pub mod pattern_matching {
+    /// `bio::pattern_matching::myers` (reference src/pattern_matching/myers): `Myers<u64>`, `Myers<u128>`,
+    /// `long::Myers` and `MyersBuilder`, with the reference's `distance`, `find_all_end` and `find_best_end` (each a
+    /// batch of one) and `*_batch` forms over many texts that store the pattern once, on the thread's engine of
+    /// `alignment::distance`.  `find_all_end` returns the hits as a `Vec` rather than a lazy iterator.
+    pub mod myers {
+        use std::collections::HashMap;
+        use std::marker::PhantomData;
+        use std::os::raw::c_void;
+
+        use crate::alignment::distance::with_engine;
+
+        #[repr(C)]
+        struct b2a_pairs {
+            seq_blob: *const u8,
+            x_off: *const u64,
+            x_len: *const u32,
+            y_off: *const u64,
+            y_len: *const u32,
+            blob_bytes: u64,
+            n_pairs: u64,
+        }
+        #[repr(C)]
+        struct b2a_myers_match {
+            ambig: *const u8,
+            wildcards: *const u8,
+        }
+        #[link(name = "b200align")]
+        extern "C" {
+            fn b2a_myers_batch(e: *mut c_void, m: *const b2a_myers_match, k: u32, pairs: *const b2a_pairs,
+                               best_end: *mut u32, best_dist: *mut u32, n_hits: *mut u64, status: *mut u32,
+                               stats: *mut c_void) -> i32;
+            fn b2a_myers_hits_fetch(e: *mut c_void, hit_off: *mut u64, hit_end: *mut u32, hit_dist: *mut u32) -> i32;
+        }
+
+        /// The bit-vector types of the simple variant: `Myers<u64>` takes patterns of up to 64 symbols, `Myers<u128>`
+        /// up to 128 (simple.rs:49-53); for `long::Myers` they only set the initial max_dist (long.rs:583-590).
+        pub trait BitVec {
+            const BITS: usize;
+        }
+        impl BitVec for u64 {
+            const BITS: usize = 64;
+        }
+        impl BitVec for u128 {
+            const BITS: usize = 128;
+        }
+
+        /// A pattern with its match relation (builder.rs): ambiguity rows (bit t of row p: pattern byte p also
+        /// matches text byte t) and text wildcards, in the tables b2a_myers_match takes.
+        #[derive(Clone)]
+        struct Searcher {
+            pattern: Vec<u8>,
+            ambig: Option<Vec<u8>>,
+            wildcards: Option<Vec<u8>>,
+        }
+
+        impl Searcher {
+            /// per text: the first end of the least distance (None for an empty text) and, with k, every
+            /// (end, distance) with distance <= k in ascending end order
+            fn search(&self, texts: &[&[u8]], k: Option<u32>) -> (Vec<Option<(usize, u32)>>, Vec<Vec<(usize, u32)>>) {
+                let n = texts.len();
+                let mut blob = self.pattern.clone();
+                let (mut y_off, mut y_len) = (Vec::with_capacity(n), Vec::with_capacity(n));
+                for t in texts {
+                    assert!(t.len() < (1usize << 31), "b200align: a text longer than 2^31 - 1");
+                    y_off.push(blob.len() as u64);
+                    y_len.push(t.len() as u32);
+                    blob.extend_from_slice(t);
+                }
+                let (x_off, x_len) = (vec![0u64; n], vec![self.pattern.len() as u32; n]);
+                let cp = b2a_pairs { seq_blob: blob.as_ptr(), x_off: x_off.as_ptr(), x_len: x_len.as_ptr(),
+                                     y_off: y_off.as_ptr(), y_len: y_len.as_ptr(), blob_bytes: blob.len() as u64,
+                                     n_pairs: n as u64 };
+                let cm = b2a_myers_match {
+                    ambig: self.ambig.as_ref().map_or(std::ptr::null(), |v| v.as_ptr()),
+                    wildcards: self.wildcards.as_ref().map_or(std::ptr::null(), |v| v.as_ptr()),
+                };
+                let (mut be, mut bd) = (vec![0u32; n], vec![0u32; n]);
+                let mut n_hits = 0u64;
+                let mut lists = vec![Vec::new(); if k.is_some() { n } else { 0 }];
+                if n > 0 {
+                    let hits_ptr: *mut u64 = if k.is_some() { &mut n_hits } else { std::ptr::null_mut() };
+                    with_engine(|e| unsafe {
+                        b2a_myers_batch(e, &cm, k.unwrap_or(0), &cp, be.as_mut_ptr(), bd.as_mut_ptr(), hits_ptr,
+                                        std::ptr::null_mut(), std::ptr::null_mut())
+                    });
+                    if k.is_some() {
+                        let mut off = vec![0u64; n + 1];
+                        let (mut he, mut hd) = (vec![0u32; n_hits as usize], vec![0u32; n_hits as usize]);
+                        with_engine(|e| unsafe { b2a_myers_hits_fetch(e, off.as_mut_ptr(), he.as_mut_ptr(), hd.as_mut_ptr()) });
+                        for (i, l) in lists.iter_mut().enumerate() {
+                            let (lo, hi) = (off[i] as usize, off[i + 1] as usize);
+                            *l = he[lo..hi].iter().zip(&hd[lo..hi]).map(|(&e, &d)| (e as usize, d)).collect();
+                        }
+                    }
+                }
+                let best = be.iter().zip(&bd).zip(texts)
+                    .map(|((&e, &d), t)| if t.is_empty() { None } else { Some((e as usize, d)) }).collect();
+                (best, lists)
+            }
+        }
+
+        /// simple.rs: patterns of at most T::BITS symbols, distances as u8
+        pub struct Myers<T: BitVec = u64> {
+            s: Searcher,
+            _t: PhantomData<T>,
+        }
+
+        impl<T: BitVec> Myers<T> {
+            pub fn new(pattern: &[u8]) -> Self {
+                MyersBuilder::new().build(pattern)
+            }
+
+            /// myers_impl.rs:163-181: u8::MAX for an empty text
+            pub fn distance_batch(&self, texts: &[&[u8]]) -> Vec<u8> {
+                self.s.search(texts, None).0.into_iter().map(|b| b.map_or(u8::MAX, |(_, d)| d as u8)).collect()
+            }
+
+            pub fn find_all_end_batch(&self, texts: &[&[u8]], max_dist: u8) -> Vec<Vec<(usize, u8)>> {
+                let lists = self.s.search(texts, Some(max_dist as u32)).1;
+                lists.into_iter().map(|l| l.into_iter().map(|(e, d)| (e, d as u8)).collect()).collect()
+            }
+
+            /// myers_impl.rs:199-207: the first end of the least distance; panics on an empty text (unwrap)
+            pub fn find_best_end_batch(&self, texts: &[&[u8]]) -> Vec<(usize, u8)> {
+                self.s.search(texts, None).0.into_iter().map(|b| b.map(|(e, d)| (e, d as u8)).unwrap()).collect()
+            }
+
+            pub fn distance(&self, text: &[u8]) -> u8 {
+                self.distance_batch(&[text])[0]
+            }
+
+            pub fn find_all_end(&self, text: &[u8], max_dist: u8) -> Vec<(usize, u8)> {
+                self.find_all_end_batch(&[text], max_dist).pop().unwrap()
+            }
+
+            pub fn find_best_end(&self, text: &[u8]) -> (usize, u8) {
+                self.find_best_end_batch(&[text])[0]
+            }
+        }
+
+        /// long.rs: patterns of any length, distances as usize
+        pub mod long {
+            use super::{BitVec, MyersBuilder, Searcher};
+            use std::marker::PhantomData;
+
+            pub struct Myers<T: BitVec = u64> {
+                pub(super) s: Searcher,
+                pub(super) _t: PhantomData<T>,
+            }
+
+            impl<T: BitVec> Myers<T> {
+                pub fn new(pattern: &[u8]) -> Self {
+                    MyersBuilder::new().build_long(pattern)
+                }
+
+                fn max_dist() -> usize {
+                    usize::MAX - T::BITS  // long.rs:583-590
+                }
+
+                pub fn distance_batch(&self, texts: &[&[u8]]) -> Vec<usize> {
+                    self.s.search(texts, None).0.into_iter().map(|b| b.map_or(Self::max_dist(), |(_, d)| d as usize)).collect()
+                }
+
+                /// max_dist.min(usize::MAX - w); a distance is at most the pattern length (< 2^31), so a bound is
+                /// passed on as at most u32::MAX without changing the hits
+                pub fn find_all_end_batch(&self, texts: &[&[u8]], max_dist: usize) -> Vec<Vec<(usize, usize)>> {
+                    let k = max_dist.min(Self::max_dist()).min(u32::MAX as usize) as u32;
+                    let lists = self.s.search(texts, Some(k)).1;
+                    lists.into_iter().map(|l| l.into_iter().map(|(e, d)| (e, d as usize)).collect()).collect()
+                }
+
+                pub fn find_best_end_batch(&self, texts: &[&[u8]]) -> Vec<(usize, usize)> {
+                    self.s.search(texts, None).0.into_iter().map(|b| b.map(|(e, d)| (e, d as usize)).unwrap()).collect()
+                }
+
+                pub fn distance(&self, text: &[u8]) -> usize {
+                    self.distance_batch(&[text])[0]
+                }
+
+                pub fn find_all_end(&self, text: &[u8], max_dist: usize) -> Vec<(usize, usize)> {
+                    self.find_all_end_batch(&[text], max_dist).pop().unwrap()
+                }
+
+                pub fn find_best_end(&self, text: &[u8]) -> (usize, usize) {
+                    self.find_best_end_batch(&[text])[0]
+                }
+            }
+        }
+
+        /// builder.rs: ambiguous pattern symbols and text wildcards
+        #[derive(Default, Clone)]
+        pub struct MyersBuilder {
+            ambigs: HashMap<u8, Vec<u8>>,
+            wildcards: Vec<u8>,
+        }
+
+        impl MyersBuilder {
+            pub fn new() -> MyersBuilder {
+                Self::default()
+            }
+
+            pub fn ambig(&mut self, byte: u8, equivalents: &[u8]) -> &mut Self {
+                self.ambigs.entry(byte).or_default().extend_from_slice(equivalents);
+                self
+            }
+
+            pub fn text_wildcard(&mut self, wildcard: u8) -> &mut Self {
+                self.wildcards.push(wildcard);
+                self
+            }
+
+            fn searcher(&self, pattern: &[u8]) -> Searcher {
+                let ambig = if self.ambigs.is_empty() { None } else {
+                    let mut t = vec![0u8; 256 * 32];
+                    for (&p, eqs) in &self.ambigs {
+                        for &q in eqs {
+                            t[32 * p as usize + (q >> 3) as usize] |= 1 << (q & 7);
+                        }
+                    }
+                    Some(t)
+                };
+                let wildcards = if self.wildcards.is_empty() { None } else {
+                    let mut t = vec![0u8; 32];
+                    for &q in &self.wildcards {
+                        t[(q >> 3) as usize] |= 1 << (q & 7);
+                    }
+                    Some(t)
+                };
+                Searcher { pattern: pattern.to_vec(), ambig, wildcards }
+            }
+
+            /// simple.rs:49-53
+            pub fn build<T: BitVec>(&self, pattern: &[u8]) -> Myers<T> {
+                assert!(pattern.len() <= T::BITS, "Pattern too long");
+                assert!(!pattern.is_empty(), "Pattern is empty");
+                Myers { s: self.searcher(pattern), _t: PhantomData }
+            }
+
+            pub fn build_64(&self, pattern: &[u8]) -> Myers<u64> {
+                self.build(pattern)
+            }
+
+            pub fn build_128(&self, pattern: &[u8]) -> Myers<u128> {
+                self.build(pattern)
+            }
+
+            /// long.rs:83-84
+            pub fn build_long<T: BitVec>(&self, pattern: &[u8]) -> long::Myers<T> {
+                assert!(!pattern.is_empty(), "Pattern is empty");
+                assert!(pattern.len() <= usize::MAX / 2, "Pattern too long");
+                long::Myers { s: self.searcher(pattern), _t: PhantomData }
+            }
+
+            pub fn build_long_64(&self, pattern: &[u8]) -> long::Myers<u64> {
+                self.build_long(pattern)
+            }
+
+            pub fn build_long_128(&self, pattern: &[u8]) -> long::Myers<u128> {
+                self.build_long(pattern)
             }
         }
     }
