@@ -469,6 +469,43 @@ int32_t b2a_multi_myers_batch(b2a_multi* m, const b2a_myers_match* match, uint32
                               b2a_stats* stats);
 int32_t b2a_multi_myers_hits_fetch(b2a_multi* m, uint64_t* hit_off, uint32_t* hit_end, uint32_t* hit_dist);
 
+/* ---- bio::stats::pairhmm::PairHMM::prob_related (reference src/stats/pairhmm/pairhmm.rs) over a batch of (x, y) pairs:
+ * the probability, summed over every alignment, that y is related to x, as a natural-log LogProb in f64.
+ * prob[p] is pair p's result, in caller order, capped at 0 (ln_one) as the reference caps it.
+ * Gap parameters are natural logs (GapParameters); free_start_gap_x / free_end_gap_x are StartEndGapParameters, with
+ * prob_start_gap_x the trait's default.  max_edit_dist UINT64_MAX is None; any other value bands the recursion as the
+ * reference does (Some(usize::MAX) gives the same results as None).
+ * Emissions come in per-base classes: every sequence byte has a class byte at the same offset of class_blob (NULL:
+ * every class is 0).  prob_emit_xy(i, j) = emit_match[cls(y[j])] when x[i] == y[j], else emit_mismatch[cls(y[j])];
+ * prob_emit_x(i) = emit_x[cls(x[i])]; prob_emit_y(j) = emit_y[cls(y[j])].  A class byte >= n_classes is B2A_E_INVALID.
+ * A gap parameter on which PairHMM::new's ln_one_minus_exp asserts (p <= 0.0) is B2A_E_INVALID.  A NaN result (the
+ * reference's assert!(!p.is_nan())) is B2A_PAIR_PANIC in `status`, prob[p] NaN; without a status array it fails the
+ * call with B2A_E_INVALID naming the pair.  Pairs with an empty side are answered on the host.
+ * A warp per pair, lanes over y (strips of 256 columns beyond 256); several pairs may share one x offset (one window,
+ * many reads).  stats: cells = sum of len_x * len_y (banded calls too: the band changes results, not the work),
+ * fill_ms = the kernels, kernel_launches.
+ * The multi form splits the pair list as b2a_multi_levenshtein_batch does; each device writes its share of prob (and
+ * status) straight into the caller's arrays. */
+typedef struct b2a_pairhmm_params {
+  double prob_gap_x, prob_gap_y, prob_gap_x_extend, prob_gap_y_extend; /* GapParameters, natural log */
+  int32_t free_start_gap_x, free_end_gap_x;                            /* StartEndGapParameters */
+  uint64_t max_edit_dist;            /* UINT64_MAX = None */
+  uint32_t n_classes;                /* 1 .. 256 */
+  const double* emit_match;          /* [n_classes] each */
+  const double* emit_mismatch;
+  const double* emit_x;
+  const double* emit_y;
+  const uint8_t* class_blob;         /* NULL, or blob_bytes class bytes laid out like seq_blob */
+} b2a_pairhmm_params;
+int32_t b2a_pairhmm_batch(b2a_engine* e, const b2a_pairhmm_params* params, const b2a_pairs* pairs, double* prob,
+                          uint32_t* status, b2a_stats* stats);
+/* How the pairs of the last b2a_pairhmm_batch ran (a measurement aid; results do not depend on it): counts[0]
+ * answered on the host (an empty side), counts[1..5] one strip with 1, 2, 4, 5, 8 columns per lane (len_y <= 32, 64,
+ * 128, 160, 256), counts[6] strips of 256 columns.  Up to n_counts (at most 7) entries are written. */
+int32_t b2a_pairhmm_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts);
+int32_t b2a_multi_pairhmm_batch(b2a_multi* m, const b2a_pairhmm_params* params, const b2a_pairs* pairs, double* prob,
+                                uint32_t* status, b2a_stats* stats);
+
 /* Measurement utility for the int32-ALU roofline (SURVEY 8d): tera lane-ops/s of
  * independent add / min-max / add+max register chains over all SMs of the device. */
 int32_t b2a_util_int32_peak(int32_t device_id, float* tops_add, float* tops_minmax, float* tops_mixed);

@@ -16,6 +16,7 @@ SO_PATH = os.path.join(HERE, "csrc", "libb200align%s.so" % (("_" + _VARIANT) if 
 
 MIN_SCORE = -858993459
 DIST_NONE = 0xFFFFFFFF  # B2A_DIST_NONE: levenshtein without a bound; None from a bounded levenshtein
+PAIRHMM_NO_BAND = 0xFFFFFFFFFFFFFFFF  # b2a_pairhmm_params.max_edit_dist of None
 MODE_CUSTOM, MODE_GLOBAL, MODE_SEMIGLOBAL, MODE_LOCAL = 0, 1, 2, 3
 ERRORS = {-1: "B2A_E_INVALID", -2: "B2A_E_NO_DEVICE", -3: "B2A_E_CUDA", -4: "B2A_E_RANGE",
           -5: "B2A_E_CAPACITY", -6: "B2A_E_STATE", -7: "B2A_E_UNSUPPORTED"}
@@ -36,6 +37,7 @@ ABI_SYMBOLS = [
     "b2a_multi_align_batch_banded_scores",
     "b2a_levenshtein_batch", "b2a_hamming_batch", "b2a_distance_tier_pairs", "b2a_multi_levenshtein_batch", "b2a_multi_hamming_batch",
     "b2a_myers_batch", "b2a_myers_hits_fetch", "b2a_myers_tier_pairs", "b2a_multi_myers_batch", "b2a_multi_myers_hits_fetch",
+    "b2a_pairhmm_batch", "b2a_pairhmm_tier_pairs", "b2a_multi_pairhmm_batch",
     "b2a_util_int32_peak",
 ]
 
@@ -70,6 +72,15 @@ class CBandHints(C.Structure):
 class CMyersMatch(C.Structure):
     """b2a_myers_match (include/b200align.h): 256 x 32-byte ambiguity rows and a 32-byte wildcard set, each or NULL"""
     _fields_ = [("ambig", C.c_void_p), ("wildcards", C.c_void_p)]
+
+
+class CPairHmmParams(C.Structure):
+    """b2a_pairhmm_params (include/b200align.h)"""
+    _fields_ = [("prob_gap_x", C.c_double), ("prob_gap_y", C.c_double), ("prob_gap_x_extend", C.c_double),
+                ("prob_gap_y_extend", C.c_double), ("free_start_gap_x", C.c_int32), ("free_end_gap_x", C.c_int32),
+                ("max_edit_dist", C.c_uint64), ("n_classes", C.c_uint32), ("emit_match", C.c_void_p),
+                ("emit_mismatch", C.c_void_p), ("emit_x", C.c_void_p), ("emit_y", C.c_void_p),
+                ("class_blob", C.c_void_p)]
 
 
 class CResults(C.Structure):
@@ -186,6 +197,10 @@ def load():
                                                     C.POINTER(CStats)]
         getattr(L, pre + "myers_hits_fetch").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.b2a_myers_tier_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+    for name in ("b2a_pairhmm_batch", "b2a_multi_pairhmm_batch"):
+        getattr(L, name).argtypes = [C.c_void_p, C.POINTER(CPairHmmParams), C.POINTER(CPairs), C.c_void_p, C.c_void_p,
+                                     C.POINTER(CStats)]
+    L.b2a_pairhmm_tier_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
     L.b2a_util_int32_peak.argtypes = [C.c_int32, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                       C.POINTER(C.c_float)]
     for name in ABI_SYMBOLS:

@@ -76,7 +76,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
     esrc = os.path.join(CSRC, "b2a_engine.cu")
     dist_h = os.path.join(CSRC, "b2a_distance.cuh")  # engine.o, distance.o and myers.o only
     myers_h = os.path.join(CSRC, "b2a_myers.cuh")  # engine.o and myers.o only
-    if force or _stale(eo, hdrs + [esrc, dist_h, myers_h]):
+    phmm_h = os.path.join(CSRC, "b2a_pairhmm.cuh")  # engine.o and pairhmm.o only
+    if force or _stale(eo, hdrs + [esrc, dist_h, myers_h, phmm_h]):
         jobs.append([NVCC, *FLAGS, "-c", esrc, "-o", eo])
     so = os.path.join(OBJ, "banded_strip_notb.o")  # the strip fill's score-only twins, beside engine.o
     objs.append(so)
@@ -93,6 +94,11 @@ def build(force: bool = False, verbose: bool = False) -> str:
     ysrc = os.path.join(CSRC, "b2a_myers.cu")
     if force or _stale(yo, hdrs + [ysrc, dist_h, myers_h]):
         jobs.append([NVCC, *FLAGS, "-c", ysrc, "-o", yo])
+    ho = os.path.join(OBJ, "pairhmm.o")  # the pair-HMM kernels (b2a_pairhmm.cuh: their lane logic)
+    objs.append(ho)
+    hsrc = os.path.join(CSRC, "b2a_pairhmm.cu")
+    if force or _stale(ho, hdrs + [hsrc, phmm_h]):
+        jobs.append([NVCC, *FLAGS, "-c", hsrc, "-o", ho])
     mo = os.path.join(OBJ, "multi.o")
     objs.append(mo)
     msrc = os.path.join(CSRC, "b2a_multi.cu")

@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -25,6 +26,7 @@
 #include "b2a_banded_strip.cuh"
 #include "b2a_distance.cuh"
 #include "b2a_myers.cuh"
+#include "b2a_pairhmm.cuh"
 
 using namespace b2a;
 
@@ -126,6 +128,7 @@ struct b2a_engine {
   uint64_t myers_tier_pairs[MT_COUNT + 1] = {0, 0, 0, 0, 0, 0, 0};
   bool myers_held = false;  // its hit list (d_hoff, d_hend, d_hdist) stays on the device until the next call
   uint64_t myers_hits = 0;
+  uint64_t pairhmm_tier_pairs[PT_COUNT] = {0, 0, 0, 0, 0, 0, 0};  // pairs per tier of the last b2a_pairhmm_batch (PT_*)
   // packed input (b2a_align_batch_packed): the caller's "blob" is BitEnc storage of this width (0 = bytes); the
   // engine unpacks it on the device and uses its own byte offsets (eff_xoff / eff_yoff) from then on
   uint32_t packed_width = 0;
@@ -2818,6 +2821,171 @@ int32_t b2a_myers_hits_fetch(b2a_engine* e, uint64_t* hit_off, uint32_t* hit_end
 int32_t b2a_myers_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts) {
   if (!e || (!counts && n_counts)) return B2A_E_INVALID;
   for (uint32_t t = 0; t < n_counts && t <= (uint32_t)MT_COUNT; ++t) counts[t] = e->myers_tier_pairs[t];
+  return B2A_OK;
+}
+
+}  // extern "C"
+
+// ---- batched pair HMM (bio::stats::pairhmm::PairHMM::prob_related): kernels and lane logic in b2a_pairhmm.cu / .cuh
+
+extern "C" {
+
+int32_t b2a_pairhmm_batch(b2a_engine* e, const b2a_pairhmm_params* prm, const b2a_pairs* pairs, double* prob,
+                          uint32_t* status, b2a_stats* stats) {
+  if (!e || !prm || !pairs || (!prob && pairs->n_pairs)) return B2A_E_INVALID;
+  if (prm->n_classes < 1 || prm->n_classes > 256)
+    return e->fail(B2A_E_INVALID, "n_classes must be 1 .. 256");
+  if (!prm->emit_match || !prm->emit_mismatch || !prm->emit_x || !prm->emit_y)
+    return e->fail(B2A_E_INVALID, "the four emission tables are required");
+  PairHmmGap g;
+  const int bad = pairhmm_gap_cache(prm->prob_gap_x, prm->prob_gap_y, prm->prob_gap_x_extend, prm->prob_gap_y_extend,
+                                    prm->free_start_gap_x != 0, prm->free_end_gap_x != 0, prm->max_edit_dist, &g);
+  if (bad)
+    return e->fail(B2A_E_INVALID, std::string("PairHMM::new: assertion failed: p <= 0.0 (ln_one_minus_exp of ") +
+                                      kPairHmmAssertArg[bad - 1] + ")");
+  int32_t rc = dist_front(e, pairs);  // (a refused batch leaves status untouched)
+  if (rc) return rc;
+  const uint64_t n = pairs->n_pairs;
+  if (prm->class_blob && prm->n_classes < 256) {
+    for (uint64_t p = 0; p < n; ++p) {
+      const uint8_t* c[2] = {prm->class_blob + pairs->x_off[p], prm->class_blob + pairs->y_off[p]};
+      const uint32_t len[2] = {pairs->x_len[p], pairs->y_len[p]};
+      for (int side = 0; side < 2; ++side) {
+        uint8_t hi = 0;
+        for (uint32_t i = 0; i < len[side]; ++i) hi = c[side][i] > hi ? c[side][i] : hi;
+        if (hi >= prm->n_classes)
+          return e->fail(B2A_E_INVALID, "pair " + std::to_string(p) + ": class byte " + std::to_string(hi) +
+                                            " >= n_classes (" + std::to_string(prm->n_classes) + ")");
+      }
+    }
+  }
+  // the tier of every pair from len_y; tasks grouped by tier, results land by pair index
+  std::vector<uint32_t> tasks[PT_COUNT];
+  std::vector<uint32_t> done;
+  uint64_t cells = 0;
+  uint32_t maxm[PT_COUNT] = {0};
+  for (uint64_t p = 0; p < n; ++p) {
+    const uint32_t m = pairs->x_len[p], nn = pairs->y_len[p];
+    cells += (uint64_t)m * nn;
+    const int t = pairhmm_tier(m, nn);
+    if (t == PT_DONE) {
+      done.push_back((uint32_t)p);
+      continue;
+    }
+    tasks[t].push_back((uint32_t)p);
+    maxm[t] = std::max(maxm[t], m);
+  }
+  const uint64_t n_dp = n - done.size();
+  e->pairhmm_tier_pairs[PT_DONE] = done.size();
+  for (int t = 1; t < PT_COUNT; ++t) e->pairhmm_tier_pairs[t] = tasks[t].size();
+  cudaStream_t st = e->stream;
+  CK(e->d_rows.reserve(n * 8 + 8));  // the results
+  if (n_dp) {
+    rc = upload_blob(e, pairs, nullptr);
+    if (rc) return rc;
+    const uint32_t ncls = prm->n_classes;
+    std::vector<double> emit(4 * (size_t)ncls);
+    std::memcpy(emit.data(), prm->emit_match, ncls * 8);
+    std::memcpy(emit.data() + ncls, prm->emit_mismatch, ncls * 8);
+    std::memcpy(emit.data() + 2 * ncls, prm->emit_x, ncls * 8);
+    std::memcpy(emit.data() + 3 * ncls, prm->emit_y, ncls * 8);
+    CK(e->d_lut.reserve(emit.size() * 8));
+    CK(cudaMemcpyAsync(e->d_lut.p, emit.data(), emit.size() * 8, cudaMemcpyHostToDevice, st));
+    e->h2d_bytes += emit.size() * 8;
+    if (prm->class_blob) {
+      CK(e->d_codemap.reserve(pairs->blob_bytes + 16));
+      if (pairs->blob_bytes)
+        CK(cudaMemcpyAsync(e->d_codemap.p, prm->class_blob, pairs->blob_bytes, cudaMemcpyHostToDevice, st));
+      e->h2d_bytes += pairs->blob_bytes;
+    }
+    std::vector<uint32_t> all;
+    all.reserve(n_dp);
+    uint32_t at[PT_COUNT + 1] = {0};
+    for (int t = 1; t < PT_COUNT; ++t) {
+      at[t] = (uint32_t)all.size();
+      all.insert(all.end(), tasks[t].begin(), tasks[t].end());
+    }
+    CK(e->d_order.reserve(all.size() * 4 + 4));
+    CK(cudaMemcpyAsync(e->d_order.p, all.data(), all.size() * 4, cudaMemcpyHostToDevice, st));
+    e->h2d_bytes += all.size() * 4;
+    CK(e->d_ctl.reserve(2048));
+    CK(cudaMemsetAsync(e->d_ctl.p, 0, 4 * PT_COUNT, st));  // one pair counter per tier
+    // per resident warp: the strip tier's boundary records (len_x each), and the semiglobal end's 3 * len_x values;
+    // the tiers run one after the other and share the two scratch buffers
+    int ctas[PT_COUNT] = {0}, wpc = 0;
+    uint64_t rec_stride[PT_COUNT] = {0}, cols_stride[PT_COUNT] = {0}, rec_bytes = 0, cols_bytes = 0;
+    size_t fr = 0, tot = 0;
+    CK(cudaMemGetInfo(&fr, &tot));
+    const uint64_t budget = e->tb_budget ? e->tb_budget : (uint64_t)((double)fr * 0.6);
+    for (int t = 1; t < PT_COUNT; ++t) {
+      if (tasks[t].empty()) continue;
+      CK(pairhmm_grid(t, e->num_sms, (uint32_t)tasks[t].size(), &ctas[t], &wpc));
+      rec_stride[t] = t == PT_STRIP ? maxm[t] : 0;
+      cols_stride[t] = g.free_end ? 3 * (uint64_t)maxm[t] : 0;
+      const uint64_t per_warp = rec_stride[t] * sizeof(PairHmmRec) + cols_stride[t] * 8;
+      if (per_warp) {  // fewer persistent warps when their scratch would not fit
+        const uint64_t fit_ctas = budget / (per_warp * wpc);
+        if (fit_ctas == 0)
+          return e->fail(B2A_E_CAPACITY, "a pair's scratch (" + std::to_string(per_warp) +
+                                             " bytes per warp) is above the device-memory budget");
+        ctas[t] = (int)std::min<uint64_t>((uint64_t)ctas[t], fit_ctas);
+      }
+      const uint64_t warps = (uint64_t)ctas[t] * wpc;
+      rec_bytes = std::max(rec_bytes, warps * rec_stride[t] * sizeof(PairHmmRec));
+      cols_bytes = std::max(cols_bytes, warps * cols_stride[t] * 8);
+    }
+    CK(e->d_bnd.reserve(rec_bytes + 16));
+    CK(e->d_bslab.reserve(cols_bytes + 16));
+    PairHmmArgs a{};
+    a.seq = e->d_blob.as<uint8_t>();
+    a.cls = prm->class_blob ? e->d_codemap.as<uint8_t>() : nullptr;
+    a.x_off = e->d_xoff.as<uint64_t>();
+    a.x_len = e->d_xlen.as<uint32_t>();
+    a.y_off = e->d_yoff.as<uint64_t>();
+    a.y_len = e->d_ylen.as<uint32_t>();
+    a.n_classes = ncls;
+    a.emit = e->d_lut.as<double>();
+    a.g = g;
+    a.prob = e->d_rows.as<double>();
+    a.rec = e->d_bnd.as<PairHmmRec>();
+    a.cols = e->d_bslab.as<double>();
+    CK(cudaEventRecord(e->ev[1], st));
+    for (int t = 1; t < PT_COUNT; ++t) {
+      a.tasks = e->d_order.as<uint32_t>() + at[t];
+      a.n_tasks = (uint32_t)tasks[t].size();
+      if (!a.n_tasks) continue;
+      a.rec_stride = rec_stride[t];
+      a.cols_stride = cols_stride[t];
+      CK(launch_pairhmm(t, a, ctas[t], wpc, e->d_ctl.as<uint32_t>() + t, st));
+      ++e->launches;
+    }
+    CK(cudaEventRecord(e->ev[2], st));
+    CK(cudaMemcpyAsync(prob, e->d_rows.p, n * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  for (uint32_t p : done) prob[p] = pairhmm_empty(pairs->x_len[p], pairs->y_len[p], prm->free_end_gap_x != 0);
+  // a NaN is the reference's assert!(!p.is_nan()): that pair only with a status array, else the call fails
+  if (!status) {
+    for (uint64_t p = 0; p < n; ++p)
+      if (std::isnan(prob[p]))
+        return e->fail(B2A_E_INVALID, "pair " + std::to_string(p) + ": assertion failed: !p.is_nan()");
+  } else {
+    for (uint64_t p = 0; p < n; ++p) status[p] = std::isnan(prob[p]) ? B2A_PAIR_PANIC : B2A_PAIR_OK;
+  }
+  if (stats) {
+    std::memset(stats, 0, sizeof(*stats));
+    stats->cells = cells;
+    stats->h2d_bytes = e->h2d_bytes;
+    stats->d2h_bytes = n_dp ? n * 8 : 0;
+    if (n_dp) cudaEventElapsedTime(&stats->fill_ms, e->ev[1], e->ev[2]);
+    stats->kernel_launches = e->launches;
+  }
+  return B2A_OK;
+}
+
+int32_t b2a_pairhmm_tier_pairs(const b2a_engine* e, uint64_t* counts, uint32_t n_counts) {
+  if (!e || (!counts && n_counts)) return B2A_E_INVALID;
+  for (uint32_t t = 0; t < n_counts && t < (uint32_t)PT_COUNT; ++t) counts[t] = e->pairhmm_tier_pairs[t];
   return B2A_OK;
 }
 

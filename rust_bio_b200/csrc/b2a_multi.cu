@@ -577,4 +577,48 @@ int32_t b2a_multi_myers_hits_fetch(b2a_multi* m, uint64_t* hit_off, uint32_t* hi
   return B2A_OK;
 }
 
+int32_t b2a_multi_pairhmm_batch(b2a_multi* m, const b2a_pairhmm_params* params, const b2a_pairs* pairs, double* prob,
+                                uint32_t* status, b2a_stats* stats) {
+  if (!m || !params || !pairs || (!prob && pairs->n_pairs)) return B2A_E_INVALID;
+  const bool split = m->devs.size() > 1 && pairs->n_pairs >= m->devs.size();
+  if (split && params->class_blob && params->n_classes >= 1 && params->n_classes < 256) {
+    // a class byte out of range fails the call naming the pair; a share would name it by its index in the share, so
+    // the whole batch is checked here first (offsets, then classes, in the single engine's order)
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p) {
+      const uint64_t bb = pairs->blob_bytes, xo = pairs->x_off[p], yo = pairs->y_off[p];
+      if (xo > bb || pairs->x_len[p] > bb - xo || yo > bb || pairs->y_len[p] > bb - yo)
+        return m->fail(B2A_E_INVALID, "sequence offset/length outside seq_blob");
+    }
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p) {
+      const uint64_t off[2] = {pairs->x_off[p], pairs->y_off[p]};
+      const uint32_t len[2] = {pairs->x_len[p], pairs->y_len[p]};
+      for (int side = 0; side < 2; ++side)
+        for (uint32_t i = 0; i < len[side]; ++i)
+          if (params->class_blob[off[side] + i] >= params->n_classes)
+            return m->fail(B2A_E_INVALID, "pair " + std::to_string(p) + ": class byte " +
+                                              std::to_string(params->class_blob[off[side] + i]) + " >= n_classes (" +
+                                              std::to_string(params->n_classes) + ")");
+    }
+  }
+  if (!status && split) {
+    // a NaN result fails the call naming the pair; a share would name it by its index in the share, so the shares run
+    // with statuses and the caller's index of the first panic is reported here
+    std::vector<uint32_t> st(pairs->n_pairs);
+    const int32_t rc = b2a_multi_pairhmm_batch(m, params, pairs, prob, st.data(), stats);
+    if (rc) return rc;
+    for (uint64_t p = 0; p < pairs->n_pairs; ++p)
+      if (st[p] != B2A_PAIR_OK) return m->fail(B2A_E_INVALID, "pair " + std::to_string(p) + ": assertion failed: !p.is_nan()");
+    return B2A_OK;
+  }
+  return run_split(
+      m, pairs, nullptr, stats, false,
+      [&](b2a_engine* e) { return b2a_pairhmm_batch(e, params, pairs, prob, status, stats); },
+      [&](b2a_engine* e, const Share& s, b2a_stats* st) {
+        // the share's blob starts at its lowest offset: the class bytes move with it
+        b2a_pairhmm_params ps = *params;
+        if (ps.class_blob) ps.class_blob += s.pairs.seq_blob - pairs->seq_blob;
+        return b2a_pairhmm_batch(e, &ps, &s.pairs, prob + s.lo, status ? status + s.lo : nullptr, st);
+      });
+}
+
 }  // extern "C"

@@ -7,7 +7,7 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 
 from . import _lib
-from ._lib import B2AError, CMyersMatch, CPairs, CResults, CScoring, CStats
+from ._lib import B2AError, CMyersMatch, CPairHmmParams, CPairs, CResults, CScoring, CStats
 
 Batch = Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray, np.ndarray]
 
@@ -87,7 +87,7 @@ class ScoreResults:
 
 class _BatchCalls:
     """The batch methods Engine and MultiEngine share: host arrays in, host results out.  A subclass binds the C entry
-    points (_c_align, _c_scores, _c_banded, _c_banded_scores, _c_levenshtein, _c_hamming, _c_myers, _c_myers_fetch: the handle's calls, each returning the rc) and _check."""
+    points (_c_align, _c_scores, _c_banded, _c_banded_scores, _c_levenshtein, _c_hamming, _c_myers, _c_myers_fetch, _c_pairhmm: the handle's calls, each returning the rc) and _check."""
 
     @staticmethod
     def _cpairs(batch: Batch):
@@ -237,6 +237,37 @@ class _BatchCalls:
             out.update(hit_off=off, hit_end=he[:h], hit_dist=hd[:h])
         return out
 
+    def pairhmm_batch(self, batch: Batch, gap, emit, free_start_gap_x: bool, free_end_gap_x: bool,
+                      max_edit_dist: Optional[int] = None, classes: Optional[np.ndarray] = None,
+                      pair_status: bool = True):
+        """b2a_pairhmm_batch: per pair, PairHMM::prob_related (bio::stats::pairhmm) of x and y -> float64 natural-log
+        probabilities in the caller's pair order, and with pair_status the B2A_PAIR_* statuses (a NaN result, the
+        reference's assert, is B2A_PAIR_PANIC).  gap: (prob_gap_x, prob_gap_y, prob_gap_x_extend, prob_gap_y_extend)
+        as natural logs.  emit: four sequences (match, mismatch, x, y) of one natural-log value per class.  classes:
+        None (every class 0) or uint8 class bytes laid out like the batch's blob.  max_edit_dist None: no band.
+        pair_status=False: a NaN result fails the call (B2AError) and only the probabilities are returned."""
+        tab = np.ascontiguousarray(np.asarray(emit, dtype=np.float64))
+        if tab.ndim != 2 or tab.shape[0] != 4 or not 1 <= tab.shape[1] <= 256:
+            raise ValueError("emit must be 4 tables of 1 .. 256 classes")
+        med = _lib.PAIRHMM_NO_BAND if max_edit_dist is None else int(max_edit_dist)
+        if not 0 <= med <= _lib.PAIRHMM_NO_BAND:
+            raise ValueError("max_edit_dist must fit in u64")
+        if classes is not None:
+            classes = np.ascontiguousarray(classes, dtype=np.uint8)
+            if classes.nbytes < batch[0].nbytes:
+                raise ValueError("classes must hold one byte per blob byte")
+        p = lambda a: a.ctypes.data_as(C.c_void_p)
+        ncls = tab.shape[1]
+        prm = CPairHmmParams(*[float(v) for v in gap], 1 if free_start_gap_x else 0, 1 if free_end_gap_x else 0, med,
+                             ncls, p(tab[0]), p(tab[1]), p(tab[2]), p(tab[3]),
+                             p(classes) if classes is not None else None)
+        n = len(batch[2])
+        out = np.zeros(max(1, n), dtype=np.float64)
+        st = np.zeros(max(1, n), dtype=np.uint32) if pair_status else None
+        cp = self._cpairs(batch)
+        self._check(self._c_pairhmm(C.byref(prm), C.byref(cp), p(out), p(st) if pair_status else None))
+        return (out[:n], st[:n]) if pair_status else out[:n]
+
 
 def myers_match(ambig=None, wildcards=None):
     """(CMyersMatch or None, the arrays it points to): the bit tables of b2a_myers_match from {pattern byte:
@@ -324,6 +355,13 @@ class Engine(_BatchCalls):
         self._check(self._L.b2a_myers_tier_pairs(self._h, buf.ctypes.data_as(C.c_void_p), 7))
         return [int(v) for v in buf]
 
+    def pairhmm_tier_pairs(self) -> list:
+        """Pairs of the last pairhmm_batch per tier: [host-answered, one strip with 1, 2, 4, 5, 8 columns per lane (5
+        entries), strips of 256 columns] (b2a_pairhmm_tier_pairs; a measurement aid)."""
+        buf = np.zeros(7, dtype=np.uint64)
+        self._check(self._L.b2a_pairhmm_tier_pairs(self._h, buf.ctypes.data_as(C.c_void_p), 7))
+        return [int(v) for v in buf]
+
     def distance_tier_pairs(self) -> list:
         """Pairs of the last levenshtein_batch per tier: [host-answered, register tier with 1..4 words (4 entries),
         4-word band, 8-word band, warp] (b2a_distance_tier_pairs; a measurement aid)."""
@@ -354,6 +392,9 @@ class Engine(_BatchCalls):
 
     def _c_myers_fetch(self, off, hit_end, hit_dist):
         return self._L.b2a_myers_hits_fetch(self._h, off, hit_end, hit_dist)
+
+    def _c_pairhmm(self, prm, cp, out, status):
+        return self._L.b2a_pairhmm_batch(self._h, prm, cp, out, status, C.byref(self.stats))
 
     def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))
@@ -554,6 +595,9 @@ class MultiEngine(_BatchCalls):
 
     def _c_myers_fetch(self, off, hit_end, hit_dist):
         return self._L.b2a_multi_myers_hits_fetch(self._h, off, hit_end, hit_dist)
+
+    def _c_pairhmm(self, prm, cp, out, status):
+        return self._L.b2a_multi_pairhmm_batch(self._h, prm, cp, out, status, C.byref(self.stats))
 
     def _c_banded_scores(self, mode, cs, k, w, cp, hints, res):
         return self._L.b2a_multi_align_batch_banded_scores(self._h, mode, cs, k, w, cp, hints, res, C.byref(self.stats))

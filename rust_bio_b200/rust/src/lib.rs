@@ -875,7 +875,7 @@ pub mod alignment {
         }
 
         /// Run `f` on this thread's engine; a failing call panics with the engine's error text (no CPU fallback).
-        /// `pattern_matching::myers` shares the engine.
+        /// `pattern_matching::myers` and `stats::pairhmm` share the engine.
         pub(crate) fn with_engine(f: impl FnOnce(*mut c_void) -> i32) {
             ENGINE.with(|cell| {
                 let mut eng = cell.borrow_mut();
@@ -1240,6 +1240,160 @@ pub mod pattern_matching {
 
             pub fn build_long_128(&self, pattern: &[u8]) -> long::Myers<u128> {
                 self.build_long(pattern)
+            }
+        }
+    }
+}
+
+// ---------------------------------------------------------------- stats, reference src/stats
+/// `bio::stats` on the GPU: the pair HMM (`pairhmm`).
+pub mod stats {
+    /// `bio::stats::pairhmm::PairHMM` (reference src/stats/pairhmm/pairhmm.rs): `prob_related` (a batch of one) and
+    /// `prob_related_batch` over many emissions sharing one set of tables, on the thread's engine of
+    /// `alignment::distance`.  Emissions come as per-base classes (`ClassEmission`); log probabilities are plain
+    /// `f64` natural logs (`LogProb`'s inner value).  Where the reference asserts (`PairHMM::new`'s
+    /// `ln_one_minus_exp`, a NaN result) this shim panics with the engine's message.
+    pub mod pairhmm {
+        use std::os::raw::c_void;
+
+        use crate::alignment::distance::with_engine;
+
+        #[repr(C)]
+        struct b2a_pairs {
+            seq_blob: *const u8,
+            x_off: *const u64,
+            x_len: *const u32,
+            y_off: *const u64,
+            y_len: *const u32,
+            blob_bytes: u64,
+            n_pairs: u64,
+        }
+        #[repr(C)]
+        struct b2a_pairhmm_params {
+            prob_gap_x: f64,
+            prob_gap_y: f64,
+            prob_gap_x_extend: f64,
+            prob_gap_y_extend: f64,
+            free_start_gap_x: i32,
+            free_end_gap_x: i32,
+            max_edit_dist: u64,
+            n_classes: u32,
+            emit_match: *const f64,
+            emit_mismatch: *const f64,
+            emit_x: *const f64,
+            emit_y: *const f64,
+            class_blob: *const u8,
+        }
+        #[link(name = "b200align")]
+        extern "C" {
+            fn b2a_pairhmm_batch(e: *mut c_void, params: *const b2a_pairhmm_params, pairs: *const b2a_pairs,
+                                 prob: *mut f64, status: *mut u32, stats: *mut c_void) -> i32;
+        }
+
+        /// GapParameters (mod.rs:140-153), natural logs
+        pub trait GapParameters {
+            fn prob_gap_x(&self) -> f64;
+            fn prob_gap_y(&self) -> f64;
+            fn prob_gap_x_extend(&self) -> f64;
+            fn prob_gap_y_extend(&self) -> f64;
+        }
+
+        /// StartEndGapParameters (mod.rs:155-179); prob_start_gap_x is the trait's default
+        pub trait StartEndGapParameters {
+            fn free_start_gap_x(&self) -> bool;
+            fn free_end_gap_x(&self) -> bool;
+        }
+
+        /// Per-base emission classes: `tables` = (emit_match, emit_mismatch, emit_x, emit_y), one natural-log value
+        /// per class (1 to 256 classes); `x_classes` / `y_classes` one class byte per base, or None for class 0.
+        pub struct ClassEmission<'a> {
+            pub x: &'a [u8],
+            pub y: &'a [u8],
+            pub tables: [&'a [f64]; 4],
+            pub x_classes: Option<&'a [u8]>,
+            pub y_classes: Option<&'a [u8]>,
+        }
+
+        pub struct PairHMM {
+            gap: [f64; 4],
+        }
+
+        impl PairHMM {
+            pub fn new<G: GapParameters>(gap_params: &G) -> Self {
+                PairHMM {
+                    gap: [gap_params.prob_gap_x(), gap_params.prob_gap_y(), gap_params.prob_gap_x_extend(),
+                          gap_params.prob_gap_y_extend()],
+                }
+            }
+
+            pub fn prob_related<A: StartEndGapParameters>(&mut self, emission: &ClassEmission, alignment_mode: &A,
+                                                          max_edit_dist: Option<usize>) -> f64 {
+                self.prob_related_batch(std::slice::from_ref(emission), alignment_mode, max_edit_dist)[0]
+            }
+
+            pub fn prob_related_batch<A: StartEndGapParameters>(&mut self, emissions: &[ClassEmission],
+                                                                alignment_mode: &A, max_edit_dist: Option<usize>)
+                                                                -> Vec<f64> {
+                let n = emissions.len();
+                let mut out = vec![0f64; n];
+                if n == 0 {
+                    return out;
+                }
+                let tables = emissions[0].tables;
+                let n_classes = tables[0].len();
+                assert!((1..=256).contains(&n_classes) && tables.iter().all(|t| t.len() == n_classes),
+                        "b200align: four emission tables of 1 .. 256 classes");
+                let (mut blob, mut cls) = (Vec::new(), Vec::new());
+                let (mut x_off, mut y_off, mut x_len, mut y_len) = (Vec::new(), Vec::new(), Vec::new(), Vec::new());
+                let with_classes = emissions.iter().any(|e| e.x_classes.is_some() || e.y_classes.is_some());
+                for e in emissions {
+                    assert!(e.tables.iter().zip(tables.iter()).all(|(a, b)| a.as_ptr() == b.as_ptr() || a == b),
+                            "b200align: every emission of a batch shares one set of tables");
+                    assert!(e.x.len() < (1usize << 31) && e.y.len() < (1usize << 31),
+                            "b200align: a sequence longer than 2^31 - 1");
+                    for (seq, c, off, len) in [(e.x, e.x_classes, &mut x_off, &mut x_len),
+                                               (e.y, e.y_classes, &mut y_off, &mut y_len)] {
+                        off.push(blob.len() as u64);
+                        len.push(seq.len() as u32);
+                        blob.extend_from_slice(seq);
+                        match c {
+                            Some(c) => {
+                                assert!(c.len() == seq.len(), "b200align: one class byte per base");
+                                cls.extend_from_slice(c)
+                            }
+                            None => cls.resize(blob.len(), 0),
+                        }
+                    }
+                }
+                let params = b2a_pairhmm_params {
+                    prob_gap_x: self.gap[0],
+                    prob_gap_y: self.gap[1],
+                    prob_gap_x_extend: self.gap[2],
+                    prob_gap_y_extend: self.gap[3],
+                    free_start_gap_x: alignment_mode.free_start_gap_x() as i32,
+                    free_end_gap_x: alignment_mode.free_end_gap_x() as i32,
+                    max_edit_dist: max_edit_dist.map_or(u64::MAX, |k| k as u64),
+                    n_classes: n_classes as u32,
+                    emit_match: tables[0].as_ptr(),
+                    emit_mismatch: tables[1].as_ptr(),
+                    emit_x: tables[2].as_ptr(),
+                    emit_y: tables[3].as_ptr(),
+                    class_blob: if with_classes { cls.as_ptr() } else { std::ptr::null() },
+                };
+                let cp = b2a_pairs {
+                    seq_blob: blob.as_ptr(),
+                    x_off: x_off.as_ptr(),
+                    x_len: x_len.as_ptr(),
+                    y_off: y_off.as_ptr(),
+                    y_len: y_len.as_ptr(),
+                    blob_bytes: blob.len() as u64,
+                    n_pairs: n as u64,
+                };
+                // no status array: a NaN result (the reference's assert) fails the call, and with_engine panics
+                with_engine(|e| unsafe {
+                    b2a_pairhmm_batch(e, &params, &cp, out.as_mut_ptr(), std::ptr::null_mut(), std::ptr::null_mut())
+                });
+                out
             }
         }
     }
